@@ -42,24 +42,8 @@ ICP_ITERS = 30
 ICP_RADIUS = 0.05
 TSDF_FRAMES = 1000
 VOXEL, RES, TRUNC_MULT, DSCALE, DMAX = 0.008, 16, 8.0, 1000.0, 3.0
-HBM_FALLBACK_GBS = 6650.0
-
-
-def measured_hbm_peak():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    except Exception:
-        return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(kernel):
-    """dram read+write bytes per launch from the committed ncu --set full summary, or None."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            return json.load(f).get(kernel)
-    except Exception:
-        return None
+HBM_PEAK_GBS, HBM_PEAK_SOURCE = 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
+DUMP_BLOCKS = 256        # voxel blocks per volume in --dump-outputs: a seeded sample keeps the dump far below 64 MB
 
 
 def icp_algorithmic_bytes(n, m):
@@ -76,7 +60,7 @@ def tsdf_algorithmic_bytes(blocks, color, width=640, height=480):
 
 
 class ClockSampler:
-    """Samples SM clocks / throttle reasons during the timed region (B200_PROFILING.md): NVML in-process
+    """Samples SM clocks / throttle reasons during the timed region: NVML in-process
     every 5 ms (the timed region is tens of milliseconds), nvidia-smi as a fallback."""
 
     def __init__(self, index=0):
@@ -445,7 +429,11 @@ def main():
                     help="also run BASELINE configs[3] once (multi-scale ColoredICP, 3 scales, 5M points, source split over the "
                          "ranks); always on for N > 1")
     ap.add_argument("--config3-points", type=int, default=5_000_000)
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -488,7 +476,7 @@ def main():
     def flush_l2():
         flush_buf.fill_(1)
 
-    peak, peak_src = measured_hbm_peak()
+    peak, peak_src = HBM_PEAK_GBS, HBM_PEAK_SOURCE
 
     # ------------------------------------------------------------------ ICP
     src, tgt, nrm, T_gt = make_icp_pair(ICP_POINTS, seed=2)
@@ -542,6 +530,9 @@ def main():
         barrier()
     icp_wall = time.perf_counter() - wall0
     icp_launches = L.launch_count() - launches0
+    dumps = {}
+    if args.dump_outputs:
+        dumps = icp_outputs(L, h, res, n, torch, stream)
     step_ms = max_over_ranks(step_ms)
     loop_ms = max_over_ranks(loop_ms)
     icp_value = world * ICP_ITERS * args.steps / (step_ms * 1e-3)
@@ -549,7 +540,7 @@ def main():
     alg = icp_algorithmic_bytes(n, m)
     icp_roof = {"bound": "hbm", "kernel": "icp_iteration_kernel", "achieved": alg / (kern_ms * 1e-3) / 1e9,
                 "peak": peak, "unit": "GB/s", "frac": alg / (kern_ms * 1e-3) / 1e9 / peak,
-                "traffic": ncu_traffic("icp_iteration_kernel"), "algorithmic_bytes_per_launch": alg,
+                "algorithmic_bytes_per_launch": alg,
                 "avg_launch_us": kern_ms * 1e3, "peak_source": peak_src}
     final = {"fitness": res.fitness, "inlier_rmse": res.inlier_rmse, "num_iterations": res.num_iterations,
              "transformation_error_vs_ground_truth": float(np.abs(np.array(res.transformation).reshape(4, 4) - T_gt).max())}
@@ -644,7 +635,7 @@ def main():
     # ----------------------------------------------------------------- TSDF
     tsdf = None
     if not args.skip_tsdf:
-        tsdf = bench_tsdf(args, rank, world, local_rank, L, torch, stream, barrier, max_over_ranks, peak, peak_src)
+        tsdf = bench_tsdf(args, rank, world, local_rank, L, torch, stream, barrier, max_over_ranks, peak, peak_src, dumps)
 
     # ---------------------------------------------------------- CPU baseline
     cpu = None
@@ -683,12 +674,73 @@ def main():
         else:
             line = dict(icp_line, tsdf=tsdf)
         print(json.dumps(line), flush=True)
+    if args.dump_outputs and rank == 0:
+        write_dumps(args.dump_outputs, dumps)
     if world > 1:
         comm.close()
         dist.destroy_process_group()
 
 
-def bench_tsdf(args, rank, world, local_rank, L, torch, stream, barrier, max_over_ranks, peak, peak_src):
+def icp_outputs(L, h, res, n, torch, stream):
+    """--dump-outputs, ICP: the o3db_icp_result of the last timed step, plus the correspondence set and per-iteration
+    (fitness, inlier_rmse) of one more registration identical to it (the path is bit-reproducible; checked here)."""
+    corr = torch.empty(n, dtype=torch.int64, device="cuda")
+    per_iter = np.zeros((ICP_ITERS, 2))
+    again = L.IcpResult()
+    L.check(L.lib.o3db_icp_reset(h, stream))
+    L.check(L.lib.o3db_icp_iterate(h, ICP_ITERS, stream))
+    L.check(L.lib.o3db_icp_finish(h, C.byref(again), corr.data_ptr(), L.dptr(per_iter), stream))
+    torch.cuda.synchronize()
+    last = np.array(res.transformation).reshape(4, 4)
+    if not (np.array_equal(np.array(again.transformation).reshape(4, 4), last) and again.fitness == res.fitness
+            and again.inlier_rmse == res.inlier_rmse):
+        raise RuntimeError("ICP registration is not reproducible: the dumped correspondences would not be the timed step's")
+    return {"icp_transformation": last,
+            "icp_fitness_rmse_iterations": np.array([res.fitness, res.inlier_rmse, res.num_iterations], np.float64),
+            "icp_per_iteration_fitness_rmse": per_iter,
+            "icp_correspondences": corr.cpu().numpy().astype(np.float64)}
+
+
+def tsdf_outputs(L, v, color, torch, stream):
+    """--dump-outputs, TSDF: the number of active blocks and DUMP_BLOCKS of them picked by a fixed seed after sorting by
+    block key (the hash table's slot order is not deterministic): keys, tsdf, weight (and colour) of every voxel."""
+    from open3d_b200.t._libshim import device_view
+    n = L.check(L.lib.o3db_vbg_size(v, stream))
+    idx = torch.empty(n, dtype=torch.int32, device="cuda")
+    L.check(L.lib.o3db_vbg_active_indices(v, idx.data_ptr(), n, stream))
+    idx = idx.long()
+    cap, vox = int(L.lib.o3db_vbg_capacity(v)), RES ** 3
+    keys = device_view(L.lib.o3db_vbg_key_buffer(v), (cap, 3), torch.int32)[idx].cpu().numpy()
+    order = np.lexsort((keys[:, 2], keys[:, 1], keys[:, 0]))
+    pick = order[np.sort(np.random.default_rng(0).choice(n, min(n, DUMP_BLOCKS), replace=False))]
+    sel = idx[torch.from_numpy(pick).cuda()]
+
+    def u16(ptr, shape):
+        return device_view(ptr, shape, torch.uint16).view(torch.int16)[sel].cpu().numpy().view(np.uint16).astype(np.float32)
+    name = "tsdf_depth_color" if color else "tsdf_depth_only"
+    out = {f"{name}_block_count": np.array([n], np.float64),
+           f"{name}_keys": keys[pick].astype(np.float64),
+           f"{name}_tsdf": device_view(L.lib.o3db_vbg_tsdf_buffer(v), (cap, vox), torch.float32)[sel].cpu().numpy(),
+           f"{name}_weight": u16(L.lib.o3db_vbg_weight_buffer(v), (cap, vox))}
+    if color:
+        out[f"{name}_color"] = u16(L.lib.o3db_vbg_color_buffer(v), (cap, vox, 3))
+    return out
+
+
+def write_dumps(path, dumps):
+    """Checks every array's dtype and the 64 MB budget first, and writes nothing unless all of it holds."""
+    bad = [name for name, a in dumps.items() if a.dtype not in (np.float32, np.float64)]
+    if bad:
+        raise ValueError(f"--dump-outputs: arrays must be float32 or float64, not {bad}")
+    total = sum(a.nbytes for a in dumps.values())
+    if total > 64 << 20:
+        raise ValueError(f"--dump-outputs: {total} bytes exceed the 64 MB budget")
+    os.makedirs(path, exist_ok=True)
+    for name, a in dumps.items():
+        np.save(os.path.join(path, f"{name}.npy"), a)
+
+
+def bench_tsdf(args, rank, world, local_rank, L, torch, stream, barrier, max_over_ranks, peak, peak_src, dumps):
     from tests.synth import PRIMESENSE_K, camera_pose, render_depth
     F = args.tsdf_frames
     mine = list(range(rank, F, world))                      # frames round-robin over independent volumes
@@ -756,6 +808,8 @@ def bench_tsdf(args, rank, world, local_rank, L, torch, stream, barrier, max_ove
                         L.check(L.lib.o3db_vbg_exec_stats(v, C.byref(em), C.byref(el), 1, stream))
                         exec_ms += em.value
                         exec_launches += el.value
+                        if args.dump_outputs and rank == 0 and it == warmup + steps - 1:
+                            dumps.update(tsdf_outputs(L, v, color, torch, stream))
                 if profiled:
                     if True:
                         tm, im, nf = C.c_double(0), C.c_double(0), C.c_int64(0)
@@ -806,14 +860,12 @@ def bench_tsdf(args, rank, world, local_rank, L, torch, stream, barrier, max_ove
                                                 "overlap, so each interval also contains an un-hidden launch latency); "
                                                 "avg_exec_us_device_timer: %globaltimer of the last CTA's end minus the earliest "
                                                 "CTA's start, accumulated by the kernel itself during the TIMED passes",
-                                 "traffic": ncu_traffic("integrate_kernel_color" if color else "integrate_kernel"),
                                  "algorithmic_bytes_per_launch": alg, "avg_launch_us": k_ms * 1e3,
                                  "touch_kernel_avg_us": 1e3 * dev["touch_ms"] / max(dev["profiled_frames"], 1),
                                  "mean_touched_blocks_per_frame": mean_blocks, "peak_source": peak_src,
                                  "model_note": "algorithmic bytes = every voxel of every touched block read AND written "
                                                "(SURVEY 8d): an upper bound, voxels behind the truncation band are read "
-                                               "but not written; `traffic` is the ncu cold-cache DRAM figure (writes still "
-                                               "in L2 at the end of a replay are not counted by ncu)",
+                                               "but not written",
                                  "frame_frac_end_to_end": alg / (dev["ms_per_frame"] * 1e-3) / 1e9 / peak}
     # slam::Model::SynthesizeModelFrame (EstimateRange + RayCast of the last frame's frustum, depth + colour),
     # SURVEY 8f #4: reported beside the integration numbers, not part of `value`

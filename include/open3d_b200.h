@@ -1,5 +1,5 @@
 /*
- * open3d_b200.h — C ABI of the B200-native ICP + TSDF hot path.
+ * open3d_b200.h — C ABI of the H100-native ICP + TSDF hot path.
  *
  * This is the drop-in boundary: a flat extern "C" surface (plain pointers and
  * sizes, no torch / Open3D types) that Open3D's L2 "thin dispatch" functions

@@ -11,7 +11,7 @@
 // Two build modes:
 //   * inside Open3D (BUILD_CUDA_MODULE build): add this file to the CUDA module instead of the bodies it replaces;
 //     core::Tensor etc. are the real classes, the stream is core::cuda::GetStream().
-//   * stand-alone check (integration/Makefile, -DO3DB_FORWARDERS_STANDALONE): the same source against the reference
+//   * stand-alone check (oracle/ref_shim/Makefile, -DO3DB_FORWARDERS_STANDALONE): the same source against the reference
 //     headers with the ref-shim's stub core::Tensor (oracle/ref_shim/stubs — a non-owning pointer/shape/dtype view),
 //     linked with libo3db200.so and exercised on the GPU by tests/test_forwarders_gpu.py through forwarder_hooks.cpp.
 // Float64 point clouds are outside this library's scope (north_star: fp32): those calls raise, exactly like any other

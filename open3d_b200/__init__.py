@@ -1,4 +1,4 @@
-"""open3d_b200 — B200-native (sm_100a) implementation of the two dense-geometry
+"""open3d_b200 — H100-native (sm_90a) implementation of the two dense-geometry
 hot paths of Open3D's tensor pipelines: point-to-plane ICP
 (``t.pipelines.registration``) and VoxelBlockGrid TSDF integration
 (``t.pipelines.slam`` / ``t.geometry.VoxelBlockGrid``).

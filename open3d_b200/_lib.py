@@ -20,7 +20,7 @@ UNIQUE_ID_BYTES = 128
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} not found. Build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-        "or open3d_b200/csrc/build.sh (needs nvcc, sm_100a). open3d_b200 has no CPU fallback.")
+        "or open3d_b200/csrc/build.sh (needs nvcc, sm_90a). open3d_b200 has no CPU fallback.")
 
 lib = C.CDLL(LIB_PATH)
 

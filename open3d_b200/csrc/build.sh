@@ -1,10 +1,11 @@
 #!/bin/bash
-# Builds libo3db200.so (sm_100a only) in-tree next to the python package.
+# Builds libo3db200.so (sm_90a only) in-tree next to the python package.
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 OUT="${HERE}/../libo3db200.so"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17
+ARCH=(-gencode arch=compute_90a,code=sm_90a)
+FLAGS=("${ARCH[@]}" -lineinfo -O3 -std=c++17
        -Xcompiler -fPIC,-ffp-contract=off,-Wall,-Wno-unused-function
        --expt-relaxed-constexpr ${O3DB_NVCC_EXTRA:-})
 cd "${HERE}"
@@ -16,6 +17,6 @@ for f in common icp tsdf comm pointcloud raycast odometry; do
   OBJS+=("${f}.o")
 done
 for p in "${PIDS[@]}"; do wait "$p"; done
-"${NVCC}" -shared -o "${OUT}" "${OBJS[@]}" -ldl
+"${NVCC}" "${ARCH[@]}" -shared -o "${OUT}" "${OBJS[@]}" -ldl
 rm -f "${OBJS[@]}"
 echo "built ${OUT}"

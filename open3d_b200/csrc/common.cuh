@@ -1,4 +1,4 @@
-// common.cuh — shared helpers of the sm_100a kernels (error plumbing, launch
+// common.cuh — shared helpers of the sm_90a kernels (error plumbing, launch
 // accounting, warp primitives).  Product code; never includes anything from
 // oracle/.
 #pragma once
@@ -53,9 +53,9 @@ inline int num_sms() {
     static int sms = 0;
     if (sms == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+        if (cudaGetDevice(&dev) != cudaSuccess) return 132;
         if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-            sms = 148;
+            sms = 132;
     }
     return sms;
 }

@@ -1,5 +1,5 @@
 // icp.cu — correspondence search, pose reduction and the fused device-resident
-// point-to-plane ICP loop for sm_100a.  See include/open3d_b200.h for the
+// point-to-plane ICP loop for sm_90a.  See include/open3d_b200.h for the
 // reference interfaces each entry point replaces and DESIGN.md for the design.
 //
 // No CPU fallback: every entry point needs a CUDA device.
@@ -873,7 +873,7 @@ struct IcpArgs {
     const float4* tcg;    // per sorted target point: colour gradient xyz, .w = intensity
     const float* sint;    // per sorted source point: intensity
     float sqrt_lg, sqrt_lp;
-    long long* dbg;       // -DICP_TIMING=1 builds only: 8 timestamps per block (see profiles/icp_timing.py)
+    long long* dbg;       // -DICP_TIMING=1 builds only: 8 timestamps per block
     // multi-GPU, in-kernel exchange (use_peer != 0): every rank's mailbox as mapped into this process
     PeerView peer;
     int use_peer;
@@ -889,10 +889,10 @@ __device__ void set_identity(double* T, float* Uf) {
 
 #ifndef ICP_STAGED_THREADS
 #define ICP_STAGED_THREADS 768   // threads per block of the staged iteration kernel: ONE fat block of 24 warps per SM (80 registers
-                                 // x 768 threads fills the register file).  Measured against 3 blocks of 256 threads per SM
-                                 // (-DICP_STAGED_THREADS=256): 53.1 vs 56.0 us per iteration at 2M points — a third of the
-                                 // per-block partial rows for the last block to add up (148 instead of 444) and a third of
-                                 // the block prologues / epilogues; the loop itself has no block-wide barrier either way.
+                                 // x 768 threads fills the register file): a third of the per-block partial rows for the last
+                                 // block to add up (one per SM instead of three) and a third of the block prologues / epilogues;
+                                 // the loop itself has no block-wide barrier either way.  On an H100 it is the fastest of
+                                 // 256 / 512 / 768 (profiles/icp_ab.py, profiles/h100_icp_ab.jsonl).
 #endif
 static constexpr int kIcpT = ICP_STAGED_THREADS;
 #ifndef ICP_DEFER
@@ -1981,7 +1981,7 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     // fitness denominator over all ranks
     c->n_total = (double)n;
     // 1 = direct (every load where it is needed), 2 = staged (TMA bulk copies + cp.async gathers one chunk
-    // ahead).  Default: whichever measured faster on B200 (DESIGN.md §4.1).
+    // ahead).  Default: staged, 1.6 % faster than direct on an H100 (DESIGN.md §4.1, profiles/h100_icp_ab.jsonl).
     c->variant = options->search_variant == 1 ? 1 : (options->search_variant == 2 ? 2 : ICP_DEFAULT_VARIANT);
     int occ = 1;
     for (int mode = 0; mode < 2; ++mode)

@@ -1,4 +1,4 @@
-// odometry.cu — RGB-D odometry, PointToPlane method, for sm_100a (SURVEY.md 8f #2): what
+// odometry.cu — RGB-D odometry, PointToPlane method, for sm_90a (SURVEY.md 8f #2): what
 // slam::Model::TrackFrameToModel runs between RayCast and Integrate in the dense-SLAM loop.
 //
 // Reference: t/pipelines/odometry/RGBDOdometry.cpp:56-206 (RGBDOdometryMultiScale / ...PointToPlane driver),

@@ -1,4 +1,4 @@
-// pointcloud.cu — t::geometry::PointCloud::VoxelDownSample for sm_100a (SURVEY.md 8f #1: the
+// pointcloud.cu — t::geometry::PointCloud::VoxelDownSample for sm_90a (SURVEY.md 8f #1: the
 // pyramid build that sits directly in front of the ICP loop, Registration.cpp:237-240, 266-269).
 //
 // Reference (t/geometry/PointCloud.cpp:496-560): voxel = floor(p / voxel_size) (f32), a HashSet

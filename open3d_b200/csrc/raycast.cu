@@ -1,4 +1,4 @@
-// raycast.cu — VoxelBlockGrid::RayCast for sm_100a (SURVEY.md 8f #4): the step after Integrate in
+// raycast.cu — VoxelBlockGrid::RayCast for sm_90a (SURVEY.md 8f #4): the step after Integrate in
 // the dense-SLAM loop (slam::Model::SynthesizeModelFrame, slam/Model.cpp:38-66).
 //
 // Reference: VoxelBlockGrid.cpp:328-402 -> kernel::voxel_grid::EstimateRange (VoxelBlockGridImpl.h:310-555)

@@ -1,4 +1,4 @@
-// tsdf.cu — sparse voxel-block TSDF volume for sm_100a: lock-free open-addressing
+// tsdf.cu — sparse voxel-block TSDF volume for sm_90a: lock-free open-addressing
 // hash of int32x3 block keys, frustum block discovery ("touch") and the fused
 // per-voxel depth-projection / weight-fusion kernel.  See include/open3d_b200.h
 // for the reference interfaces replaced and DESIGN.md for layout + rooflines.

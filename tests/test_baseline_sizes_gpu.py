@@ -197,11 +197,6 @@ def test_config4_dense_slam_100_frames_vs_oracle_loop(o3d):
     # so the trajectories separate slowly instead of staying at rounding level (measured: <= 2e-6 over the first 6
     # frames, 1.5e-3 max over 100 frames, i.e. 3 % of the common drift).  Bars: rounding-level agreement early, 3 mm
     # anywhere, and the same drift against the ground truth to 2 mm.
-    out = os.path.join(ROOT, "gpurun_out")
-    if os.path.isdir(out):
-        with open(os.path.join(out, "slam_100_frames_vs_oracle.txt"), "w") as f:
-            f.write(f"max|pose_gpu-pose_oracle| {dev.max():.6e} at frame {int(dev.argmax())}; first 6 frames {dev[:6].max():.3e}; "
-                    f"drift_vs_gt_mm gpu {1e3 * drift_gpu[-1]:.3f} oracle {1e3 * drift_ref[-1]:.3f}\n")
     assert dev[:6].max() < 1e-4, dev[:6]
     assert dev.max() < 3e-3, (int(dev.argmax()), dev.max())
     assert abs(drift_gpu[-1] - drift_ref[-1]) < 2e-3                  # same drift to within 2 mm
@@ -251,7 +246,7 @@ def test_config3_colored_multiscale_icp_3_scales_500k_vs_oracle(o3d):
 
 # ------------------------------------------------------------------ §8(e)
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_sharded_icp_equals_single_gpu_on_2_gpus():
     """tests/multigpu_check.py under torchrun, 2 ranks over NCCL: source-sharded point-to-plane ICP and ColoredICP
     (one 30-double all-reduce per iteration inside the library) == the single-GPU run on the whole source."""

@@ -58,11 +58,10 @@ def test_product_does_not_import_oracle():
                 assert "liboracle" not in src and "orc_" not in src, f
 
 
-def test_shipped_library_carries_the_blackwell_instructions_the_design_claims():
-    """SASS of the in-tree libo3db200.so (sm_100a cubins): the TMA bulk copy of the ICP chunk ring (UBLKCP), the tiled
+def test_shipped_library_carries_the_hopper_instructions_the_design_claims():
+    """SASS of the in-tree libo3db200.so (sm_90a cubins): the TMA bulk copy of the ICP chunk ring (UBLKCP), the tiled
     TMA load of the integrate kernel (UTMALDG.2D), mbarrier transactions (SYNCS), programmatic dependent launch
-    (ACQBULK / PREEXIT) and the cluster barrier of the level-resident odometry kernel (UCGABAR) — DESIGN.md §4,
-    profiles/r02_sass_excerpts.md.  A build that silently lost one of them (a knob left on, an #if) fails here."""
+    (ACQBULK / PREEXIT) and the cluster barrier of the level-resident odometry kernel (UCGABAR) — DESIGN.md §4.  A build that silently lost one of them (a knob left on, an #if) fails here."""
     import shutil
     import subprocess
     from open3d_b200 import _lib
@@ -70,7 +69,7 @@ def test_shipped_library_carries_the_blackwell_instructions_the_design_claims():
     if not os.path.exists(tool):
         pytest.skip("cuobjdump not available")
     elfs = subprocess.run([tool, "-lelf", _lib.LIB_PATH], capture_output=True, text=True, timeout=120).stdout
-    assert "sm_100a" in elfs
+    assert "sm_90a" in elfs
     sass = subprocess.run([tool, "-sass", _lib.LIB_PATH], capture_output=True, text=True, timeout=300).stdout
     current, per_kernel = None, {}
     for line in sass.splitlines():

@@ -1,8 +1,8 @@
 """The drop-in boundary as CODE: integration/o3d_forwarders.cpp defines the reference's own `*CUDA` functions
 (signatures from the reference's headers — RegistrationImpl.h:93-131, VoxelBlockGrid.h:345-381, Transform.h:42-47,
 FixedRadiusIndex.h:227, 364 — compiled against them with the ref-shim's stub core::Tensor) as forwarders into
-libo3db200.so.  integration/_build/libo3d_forwarders.so is built by integration/Makefile in the build container
-(needs /root/reference) and travels to the GPU box.  CPU part: the library exports the reference's mangled
+libo3db200.so.  oracle/_ref/libo3d_forwarders.so is built by oracle/ref_shim/Makefile where the reference source tree
+is readable, like the rest of oracle/_ref.  CPU part: the library exports the reference's mangled
 names.  GPU part: calling those functions gives the oracle's results.
 """
 import ctypes as C
@@ -17,8 +17,8 @@ import oracle
 from tests.synth import PRIMESENSE_K, camera_pose, make_colors, make_icp_pair, render_depth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "integration", "_build", "libo3d_forwarders.so")
-needs_so = pytest.mark.skipif(not os.path.exists(SO), reason="integration/_build not built (needs /root/reference at build time)")
+SO = os.path.join(ROOT, "oracle", "_ref", "libo3d_forwarders.so")
+needs_so = pytest.mark.skipif(not os.path.exists(SO), reason="oracle/_ref not built (needs the reference source tree)")
 
 REFERENCE_SYMBOLS = [   # demangled prefixes the reference's callers link against
     "open3d::t::pipelines::kernel::ComputePosePointToPlaneCUDA(",
