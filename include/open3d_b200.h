@@ -200,7 +200,6 @@ typedef struct {
     double relative_rmse;       /* ICPConvergenceCriteria::relative_rmse_ */
     o3db_robust_kernel kernel;  /* TransformationEstimationPointToPlane::kernel_ */
     double cell_scale;          /* search-grid cell = cell_scale * radius (0 => default) */
-    int search_variant;         /* 0 = default (2); 1 = direct loads (A/B baseline); 2 = staged: TMA bulk copies + cp.async ring, DESIGN.md 4.1 */
 } o3db_icp_options;
 
 typedef struct {

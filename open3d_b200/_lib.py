@@ -32,7 +32,7 @@ class RobustKernel(C.Structure):
 class IcpOptions(C.Structure):
     _fields_ = [("max_correspondence_distance", C.c_double), ("max_iteration", C.c_int),
                 ("relative_fitness", C.c_double), ("relative_rmse", C.c_double),
-                ("kernel", RobustKernel), ("cell_scale", C.c_double), ("search_variant", C.c_int)]
+                ("kernel", RobustKernel), ("cell_scale", C.c_double)]
 
 
 class IcpResult(C.Structure):

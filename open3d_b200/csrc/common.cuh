@@ -74,23 +74,63 @@ void pinned_release(void* p);
 
 #ifdef __CUDACC__
 // Programmatic dependent launch: a kernel launched through launch_pdl_ex may become resident while its predecessor
-// on the stream drains; it must call pdl_grid_wait() before touching anything the predecessor wrote.
-__device__ __forceinline__ void pdl_grid_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_grid_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+// on the stream drains; it must call pdl_wait() before touching anything the predecessor wrote.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+// Launch shape of launch_pdl_ex.  cluster > 0: thread-block clusters of `cluster` CTAs along x.
+struct PdlLaunch {
+    dim3 grid;
+    unsigned block;
+    size_t smem = 0;
+    unsigned cluster = 0;
+};
+
+// Every kernel of the library that is ordered by griddepcontrol.wait is launched here, with the
+// programmatic-stream-serialization attribute.
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl_ex(void (*kernel)(KArgs...), unsigned grid, unsigned block, size_t smem, cudaStream_t st,
-                                 Args&&... args) {
+inline cudaError_t launch_pdl_ex(void (*kernel)(KArgs...), const PdlLaunch& l, cudaStream_t st, Args&&... args) {
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(block);
-    cfg.dynamicSmemBytes = smem;
+    cfg.gridDim = l.grid;
+    cfg.blockDim = dim3(l.block);
+    cfg.dynamicSmemBytes = l.smem;
     cfg.stream = st;
-    cudaLaunchAttribute attr[1];
+    cudaLaunchAttribute attr[2];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
+    attr[1].id = cudaLaunchAttributeClusterDimension;
+    attr[1].val.clusterDim.x = l.cluster;
+    attr[1].val.clusterDim.y = 1;
+    attr[1].val.clusterDim.z = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = 1;
+    cfg.numAttrs = l.cluster > 0 ? 2 : 1;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
+// %globaltimer: nanoseconds, comparable across the SMs of a device.
+__device__ __forceinline__ long long global_ns() {
+    long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+// mbarrier (sm_90) helpers shared by the TMA pipelines of icp.cu and tsdf.cu.
+__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(unsigned long long* b, unsigned count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(b)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long* b, unsigned bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(b)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(unsigned long long* b, unsigned parity) {
+    unsigned done;
+    do {
+        asm volatile(
+                "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                : "=r"(done)
+                : "r"(smem_u32(b)), "r"(parity)
+                : "memory");
+    } while (!done);
 }
 
 __device__ __forceinline__ double warp_sum(double v) {

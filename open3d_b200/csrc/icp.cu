@@ -20,32 +20,8 @@ namespace o3db {
 
 static constexpr int64_t kMaxCells = int64_t(1) << 26;  // 256 MB of u32 CSR offsets at most
 static constexpr int kMaxCellsPerAxis = 4096;
-#ifndef ICP_THIN_FACTOR
-#define ICP_THIN_FACTOR 8
-#endif
-static constexpr double kThinFactor = ICP_THIN_FACTOR;   // grid-x (thin axis) cells are this much coarser
-#ifndef ICP_SEEDED
-#define ICP_SEEDED 1   // 1: seed every query's search with its winner of the previous iteration (exact; see nn_search_seeded)
-#endif
-static constexpr bool kSeeded = ICP_SEEDED != 0;
-#ifndef ICP_CERTIFY
-#define ICP_CERTIFY 1   // 1: skip the scan when the triangle inequality proves last iteration's winner is still the winner
-#endif
-static constexpr bool kCertify = ICP_CERTIFY != 0;
-#ifndef ICP_CELL_SCALE
-#define ICP_CELL_SCALE 0.5
-#endif
-static constexpr double kDefaultCellScale = ICP_CELL_SCALE;
-#ifndef ICP_TWO_PASS
-#define ICP_TWO_PASS 1   // 1: slab/two-pass search on the fine grid (default), 0: pruned single-pass search
-#endif
-static constexpr bool kTwoPass = ICP_TWO_PASS != 0;
-#ifndef ICP_MIN_BLOCKS
-#define ICP_MIN_BLOCKS 3
-#endif
-#ifndef ICP_DEFAULT_VARIANT
-#define ICP_DEFAULT_VARIANT 2   // 1 = direct, 2 = staged (TMA + cp.async ring)
-#endif
+static constexpr double kThinFactor = 8;   // grid-x (thin axis) cells are this much coarser
+static constexpr double kDefaultCellScale = 0.5;   // see icp_create_impl
 
 // --------------------------------------------------------------------- bbox
 
@@ -354,9 +330,7 @@ static void nns_free(o3db_nns* s, cudaStream_t st) {
     s->cell_start = nullptr;
 }
 
-#ifndef ICP_THIN_MERGE_MAX
-#define ICP_THIN_MERGE_MAX 8.0   // merge the whole thin axis into ONE cell while a (y, z) column holds at most this many points on average
-#endif
+static constexpr double kThinMergeMax = 8.0;   // merge the whole thin axis into ONE cell while a (y, z) column holds at most this many points on average
 static int grid_from_bbox(const float mn[3], const float mx[3], double radius, double cell_scale, int64_t m, Grid* g,
                           int64_t* ncell) {
     double c = radius * (cell_scale > 0 ? cell_scale : 1.0) * (1.0 + 1e-4);
@@ -382,7 +356,7 @@ static int grid_from_bbox(const float mn[3], const float mx[3], double radius, d
         // shrinks by nx and a slab boundary is one multiply-free lookup.  Volumetric clouds keep thin cells.
         const double cols = (std::floor(ext[order[1]] / c) + 1) * (std::floor(ext[order[2]] / c) + 1);
         cx = c * kThinFactor;
-        if ((double)m <= ICP_THIN_MERGE_MAX * cols) cx = std::max(cx, ext[order[0]] * (1.0 + 1e-3) + c);
+        if ((double)m <= kThinMergeMax * cols) cx = std::max(cx, ext[order[0]] * (1.0 + 1e-3) + c);
         for (int k = 0; k < 3; ++k) {
             n[k] = std::floor(ext[order[k]] / (k == 0 ? cx : c)) + 1;
             ok = ok && n[k] <= kMaxCellsPerAxis;
@@ -873,7 +847,6 @@ struct IcpArgs {
     const float4* tcg;    // per sorted target point: colour gradient xyz, .w = intensity
     const float* sint;    // per sorted source point: intensity
     float sqrt_lg, sqrt_lp;
-    long long* dbg;       // -DICP_TIMING=1 builds only: 8 timestamps per block
     // multi-GPU, in-kernel exchange (use_peer != 0): every rank's mailbox as mapped into this process
     PeerView peer;
     int use_peer;
@@ -887,46 +860,11 @@ __device__ void set_identity(double* T, float* Uf) {
     }
 }
 
-#ifndef ICP_STAGED_THREADS
-#define ICP_STAGED_THREADS 768   // threads per block of the staged iteration kernel: ONE fat block of 24 warps per SM (80 registers
-                                 // x 768 threads fills the register file): a third of the per-block partial rows for the last
-                                 // block to add up (one per SM instead of three) and a third of the block prologues / epilogues;
-                                 // the loop itself has no block-wide barrier either way.  On an H100 it is the fastest of
-                                 // 256 / 512 / 768 (profiles/icp_ab.py, profiles/h100_icp_ab.jsonl).
-#endif
-static constexpr int kIcpT = ICP_STAGED_THREADS;
-#ifndef ICP_DEFER
-#define ICP_DEFER 1   // N > 1: a lane adds the term vectors of N consecutive chunks (f32) before the warp reduces them
-#endif
-#ifndef ICP_TRANSPOSE_SMEM
-#define ICP_TRANSPOSE_SMEM 0   // 1: the per-chunk transposed reduction goes through a shared-memory tile instead of shuffles
-#endif
-#ifndef ICP_TIMING
-#define ICP_TIMING 0   // 1: record per-block timestamps of the last iteration launch (diagnostics only)
-#endif
-__device__ __forceinline__ long long global_ns() {
-    long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-#define ICP_STAMP(slot)                                                                            \
-    do {                                                                                           \
-        if (ICP_TIMING && a.dbg && threadIdx.x == 0) a.dbg[(size_t)blockIdx.x * 8 + (slot)] = global_ns(); \
-    } while (0)
-
-#ifndef ICP_PDL
-#define ICP_PDL 1   // 1: launch the iteration kernels with programmatic stream serialization (see pdl_wait)
-#endif
-__device__ __forceinline__ void pdl_wait() {
-#if ICP_PDL
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void pdl_launch_dependents() {
-#if ICP_PDL
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-#endif
-}
+// Threads per block of the iteration kernel: ONE fat block of 24 warps per SM (80 registers x 768 threads fills the
+// register file): a third of the per-block partial rows for the last block to add up (one per SM instead of three)
+// and a third of the block prologues / epilogues; the loop itself has no block-wide barrier either way.  On an H100
+// it is faster than 256 or 512 (profiles/h100_icp_ab.jsonl).
+static constexpr int kIcpThreads = 768;
 
 // Host part of DoSingleScaleICPIterations (Registration.cpp:293-358), on device, run by ONE WARP once per
 // iteration (all 32 lanes must call it): the 6x6 solve is warp-parallel, the six sin / cos of the pose and the
@@ -1066,7 +1004,7 @@ __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float*
         const float clear = __fsub_rd(clear_prev, moved);
         const float r1 = sd > 0.f ? __fmul_ru(sd * rsqrtf(sd), 1.00001f) : 0.f;
         if (sd <= a.thr) {
-            if (kCertify && r1 < clear) {
+            if (r1 < clear) {
                 bj = (unsigned)jp;
                 clear_new = clear;
                 handled = true;
@@ -1076,13 +1014,11 @@ __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float*
         }
     }
     if (!handled) {
-        bj = nn_search_slow(&a.g, a.tgt, a.cs, p.x, p.y, p.z, kTwoPass ? a.r1 : a.rr, a.r1_accept2, a.rr, a.thr, jp);
+        bj = nn_search_slow(&a.g, a.tgt, a.cs, p.x, p.y, p.z, a.r1, a.r1_accept2, a.rr, a.thr, jp);
         clear_new = 0.f;
     }
-    if (kSeeded) {
-        if ((int)bj != jp) *a.src.seed(i) = (int)bj;
-        *a.src.clearance(i) = clear_new;
-    }
+    if ((int)bj != jp) *a.src.seed(i) = (int)bj;
+    *a.src.clearance(i) = clear_new;
     int widx = -1;
     if (bj != kNoPoint) {
         const float4 t = (int)bj == jp ? ts : __ldg(&a.tgt[bj]);   // (just scanned: an L1 hit)
@@ -1115,30 +1051,6 @@ __device__ __forceinline__ void icp_accumulate_chunk(float (&term)[32], bool mat
     if (__any_sync(0xffffffffu, matched)) acc64 += (double)warp_transpose_sum32(term);
 }
 
-// The same through a per-warp shared-memory tile (30 conflict-free STS + 8 LDS.128 + a 31-add tree instead of
-// 31 shuffles + 62 selects + 31 adds): rows are 36 floats apart, so that the 8 lanes of an LDS.128 phase hit
-// 8 different bank quads.  Same f32 association as a balanced binary tree over the lanes.
-static constexpr int kTrStride = 36;
-static constexpr int kTrFloats = kNumSums * kTrStride;
-__device__ __forceinline__ void icp_accumulate_chunk_smem(float (&term)[32], bool matched, float* tr, double& acc64) {
-    if (!__any_sync(0xffffffffu, matched)) return;
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int k = 0; k < kNumSums; ++k) tr[k * kTrStride + lane] = term[k];
-    __syncwarp();
-    if (lane < kNumSums) {
-        const float4* row = reinterpret_cast<const float4*>(tr + lane * kTrStride);
-        float q[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            const float4 v = row[k];
-            q[k] = (v.x + v.y) + (v.z + v.w);
-        }
-        acc64 += (double)(((q[0] + q[1]) + (q[2] + q[3])) + ((q[4] + q[5]) + (q[6] + q[7])));
-    }
-    __syncwarp();   // the tile is rewritten by the next chunk
-}
-
 // The exchange step of the source-sharded loop (SURVEY.md 8e), done INSIDE the iteration kernel over NVLink /
 // NVSwitch peer memory instead of kernel -> ncclAllReduce -> finalize kernel.  Flag-in-data protocol (what NCCL
 // calls LL): warp 0 of each rank's last block stores its 30 local sums into slot [parity][rank] of EVERY rank's
@@ -1168,8 +1080,7 @@ __device__ __forceinline__ bool peer_all_reduce(const PeerView& pv, double* s_fi
     }
     double acc = 0.0;
     bool ok = true;
-    long long t0;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+    const long long t0 = global_ns();
     // collect in batches of 8 ranks: all loads of a batch are in flight together (one memory round trip per batch when
     // the peers have already published, instead of one per rank), the sum stays in rank order
     constexpr int kBatch = 8;
@@ -1191,9 +1102,7 @@ __device__ __forceinline__ bool peer_all_reduce(const PeerView& pv, double* s_fi
                 for (int u = 0; u < kBatch; ++u)
                     if ((pending & (1u << u)) && (unsigned)(w0[u] >> 32) == tag && (unsigned)(w1[u] >> 32) == tag) pending &= ~(1u << u);
                 if (pending) {
-                    long long t;
-                    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-                    if (t - t0 > 4000000000ll) {   // 4 s
+                    if (global_ns() - t0 > 4000000000ll) {   // 4 s
                         ok = false;
                         break;
                     }
@@ -1213,14 +1122,11 @@ __device__ __forceinline__ bool peer_all_reduce(const PeerView& pv, double* s_fi
     return ok;
 }
 
-// Block epilogue shared by both iteration kernels: block partial -> (last block) grand total, solve,
-// pose update, convergence test.
-template <int MODE, int THREADS = kThreads>
+// Block epilogue of the iteration kernel: block partial -> (last block) grand total, solve, pose update,
+// convergence test.
+template <int MODE>
 __device__ __forceinline__ void icp_block_epilogue(const IcpArgs& a, double (*s_warp)[kSumStride], double* s_final) {
-    ICP_STAMP(2);   // this block's first warp is through its loop
-    long long* stamps = (ICP_TIMING && a.dbg) ? a.dbg + (size_t)blockIdx.x * 8 + 3 : nullptr;   // [3] all warps done, [4] ticket = last
-    if (!block_reduce_to_global<THREADS>(s_warp, a.partials, &a.st->ticket, s_final, stamps)) return;
-    ICP_STAMP(5);   // last block: grand total ready
+    if (!block_reduce_to_global<kIcpThreads>(s_warp, a.partials, &a.st->ticket, s_final)) return;
     if (a.fuse_finalize) {
         if (threadIdx.x < 32) {
             if (a.use_peer && !peer_all_reduce(a.peer, s_final)) {
@@ -1236,58 +1142,9 @@ __device__ __forceinline__ void icp_block_epilogue(const IcpArgs& a, double (*s_
     } else if (threadIdx.x < kNumSums) {
         a.st->sums[threadIdx.x] = s_final[threadIdx.x];
     }
-    ICP_STAMP(7);   // last block: solve + pose update done
 }
 
-// ------------------------------------------------ direct variant (search_variant = 1)
-
-// One ICP iteration in ONE kernel, every load issued where it is needed (source point, seed, seed's
-// normal, CSR offsets, candidates: four dependent round trips per query).  Kept as the A/B baseline of the
-// staged kernel below; same results bit for bit.
-template <bool L2LOSS, int MODE, bool COLORED = false>
-__global__ void __launch_bounds__(kThreads, ICP_MIN_BLOCKS)
-icp_iteration_direct_kernel(const __grid_constant__ IcpArgs a) {
-    __shared__ double s_warp[kThreads / 32][kSumStride];
-    __shared__ double s_final[kSumStride];
-    __shared__ float s_U[16];
-    __shared__ int s_done;
-    for (int k = threadIdx.x; k < (kThreads / 32) * kSumStride; k += kThreads) (&s_warp[0][0])[k] = 0.0;
-    ICP_STAMP(0);   // block resident
-    if (ICP_TIMING && a.dbg && threadIdx.x == 0) {
-        unsigned smid;
-        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-        a.dbg[(size_t)blockIdx.x * 8 + 6] = smid;
-    }
-    pdl_wait();
-    pdl_launch_dependents();
-    ICP_STAMP(1);   // predecessor complete
-    if (threadIdx.x == 0) s_done = *(volatile int*)&a.st->done;
-    if (threadIdx.x < 16) s_U[threadIdx.x] = a.st->Uf[threadIdx.x];
-    __syncthreads();
-    if (MODE == 0 && s_done) return;
-
-    double acc64 = 0.0;      // lane l: running total of slot l over this warp's queries
-    const int n = (int)a.n;
-    for (int base = blockIdx.x * kThreads; base < n; base += gridDim.x * kThreads) {
-        const int i = base + threadIdx.x;
-        float term[32];
-#pragma unroll
-        for (int k = 0; k < 32; ++k) term[k] = 0.f;
-        bool matched = false;
-        if (i < n) {
-            const float4 p = *a.src.point(i);
-            const int jp = kSeeded ? *a.src.seed(i) : -1;
-            const float clear_prev = kSeeded ? *a.src.clearance(i) : 0.f;
-            matched = icp_process_query<L2LOSS, MODE, COLORED>(a, s_U, i, p, jp, clear_prev, a.tgt + max(jp, 0), a.nrm + max(jp, 0),
-                                                               COLORED ? a.tcg + max(jp, 0) : nullptr, term);
-        }
-        icp_accumulate_chunk(term, matched, acc64);
-    }
-    if ((threadIdx.x & 31) < kNumSums) s_warp[threadIdx.x >> 5][threadIdx.x & 31] = acc64;
-    icp_block_epilogue<MODE>(a, s_warp, s_final);
-}
-
-// ------------------------------------------ staged variant (default): TMA + cp.async ring
+// ------------------------------------------------ iteration kernel: TMA + cp.async ring
 
 // Per warp, a two-slot ring in shared memory holds what a 32-query chunk needs before its search can
 // start, fetched while the PREVIOUS chunk is being searched:
@@ -1312,28 +1169,11 @@ struct __align__(16) IcpStage {
     float4 cg[COLORED ? 32 : 1];   // their colour rows
 };
 
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* b, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(b)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* b, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(b)), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* b) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                          smem_u32(dst)),
                  "l"(src), "r"(bytes), "r"(smem_u32(b))
                  : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* b, unsigned parity) {
-    unsigned done;
-    do {
-        asm volatile(
-                "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                : "=r"(done)
-                : "r"(smem_u32(b)), "r"(parity)
-                : "memory");
-    } while (!done);
 }
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
@@ -1343,37 +1183,27 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 
 template <bool COLORED>
 struct IcpStagedSmem {   // dynamic shared memory of icp_iteration_kernel
-    IcpStage<COLORED> stage[kIcpT / 32][2];
-#if ICP_TRANSPOSE_SMEM
-    float tr[kIcpT / 32][kTrFloats];
-#endif
+    IcpStage<COLORED> stage[kIcpThreads / 32][2];
 };
 
 template <bool L2LOSS, int MODE, bool COLORED = false>
-__global__ void __launch_bounds__(kIcpT, kIcpT >= 512 ? 1 : ICP_MIN_BLOCKS)
+__global__ void __launch_bounds__(kIcpThreads, 1)
 icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     IcpStagedSmem<COLORED>& sm = *reinterpret_cast<IcpStagedSmem<COLORED>*>(smem_raw);
-    __shared__ double s_warp[kIcpT / 32][kSumStride];
+    __shared__ double s_warp[kIcpThreads / 32][kSumStride];
     __shared__ double s_final[kSumStride];
     __shared__ float s_U[16];
     __shared__ int s_done;
-    __shared__ __align__(8) unsigned long long s_mbar[kIcpT / 32][2];
+    __shared__ __align__(8) unsigned long long s_mbar[kIcpThreads / 32][2];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    for (int k = threadIdx.x; k < (kIcpT / 32) * kSumStride; k += kIcpT) (&s_warp[0][0])[k] = 0.0;
-    if (threadIdx.x < 2 * (kIcpT / 32)) mbar_init(&s_mbar[0][0] + threadIdx.x, 1);
+    for (int k = threadIdx.x; k < (kIcpThreads / 32) * kSumStride; k += kIcpThreads) (&s_warp[0][0])[k] = 0.0;
+    if (threadIdx.x < 2 * (kIcpThreads / 32)) mbar_init(&s_mbar[0][0] + threadIdx.x, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     // Programmatic dependent launch: this grid may become resident while the previous iteration's last
     // block is still in its serial epilogue; nothing produced by that kernel is read before the wait.
-    ICP_STAMP(0);   // block resident
-    if (ICP_TIMING && a.dbg && threadIdx.x == 0) {
-        unsigned smid;
-        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-        a.dbg[(size_t)blockIdx.x * 8 + 6] = smid;
-    }
     pdl_wait();
     pdl_launch_dependents();
-    ICP_STAMP(1);   // predecessor complete
     if (threadIdx.x == 0) s_done = *(volatile int*)&a.st->done;
     if (threadIdx.x < 16) s_U[threadIdx.x] = a.st->Uf[threadIdx.x];
     __syncthreads();
@@ -1382,15 +1212,15 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     // chunk c of this warp covers working-source positions [q0(c), q0(c) + 32); the arrays are padded to
     // a multiple of 256 entries, so a chunk that starts below n can always be copied whole
     const int n = (int)a.n;
-    const int stride = gridDim.x * kIcpT;
-    const int first = blockIdx.x * kIcpT + w * 32;
+    const int stride = gridDim.x * kIcpThreads;
+    const int first = blockIdx.x * kIcpThreads + w * 32;
     constexpr unsigned kBytesA = kSrcChunkBytes;
     static_assert(offsetof(IcpStage<COLORED>, jp) == 512 && offsetof(IcpStage<COLORED>, d2) == 640, "stage A mirrors a chunk record");
     auto issue_a = [&](int c, int q0) {        // lane 0: ONE TMA bulk copy of chunk c's record into slot c & 1
         if (lane == 0 && q0 < n) {
             IcpStage<COLORED>& sl = sm.stage[w][c & 1];
             unsigned long long* mb = &s_mbar[w][c & 1];
-            mbar_expect_tx(mb, kBytesA);
+            mbar_arrive_expect_tx(mb, kBytesA);
             bulk_g2s(sl.p, a.src.chunk(q0), kBytesA, mb);
         }
     };
@@ -1398,7 +1228,7 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
         if (q0 < n) {
             IcpStage<COLORED>& sl = sm.stage[w][c & 1];
             mbar_wait(&s_mbar[w][c & 1], (unsigned)(c >> 1) & 1u);
-            const int jp = kSeeded ? sl.jp[lane] : -1;
+            const int jp = sl.jp[lane];
             if (jp >= 0) {
                 cp_async16(&sl.ts[lane], a.tgt + jp);
                 if (MODE == 0) cp_async16(&sl.ns[lane], a.nrm + jp);
@@ -1409,11 +1239,6 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     };
 
     double acc64 = 0.0;      // lane l: running total of slot l over this warp's queries
-#if ICP_DEFER > 1
-    float term[32];
-    int pending = 0;
-    bool matched = false;
-#endif
     issue_a(0, first);
     issue_a(1, first + stride);
     issue_b(0, first);
@@ -1423,29 +1248,13 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
         // A(c) has landed: every lane waited on its mbarrier in issue_b(c), one trip ago (or in the prologue)
         cp_async_wait_all();                                       // B(c)
         const float4 p = sl.p[lane];
-        const int jp = kSeeded ? sl.jp[lane] : -1;
+        const int jp = sl.jp[lane];
         const float clear_prev = sl.d2[lane];
         __syncwarp();          // every lane has read p / jp / d2 of slot c & 1: hand that part back to the producer
         issue_a(c + 2, q0 + 2 * stride);
         issue_b(c + 1, q0 + stride);
         // (ts / ns / cg of slot c & 1 are rewritten by issue_b(c + 2), i.e. in the NEXT trip: still valid below)
         const int i = q0 + lane;
-#if ICP_DEFER > 1
-        // the lane's terms of ICP_DEFER consecutive chunks are added in f32 first (fixed order: deterministic);
-        // the 150-instruction transposed warp reduction then runs once per ICP_DEFER chunks
-        if (pending == 0) {
-#pragma unroll
-            for (int k = 0; k < 32; ++k) term[k] = 0.f;
-        }
-        if (i < n)
-            matched |= icp_process_query<L2LOSS, MODE, COLORED>(a, s_U, i, p, jp, clear_prev, &sl.ts[lane], &sl.ns[lane],
-                                                                &sl.cg[COLORED ? lane : 0], term);
-        if (++pending == ICP_DEFER) {
-            icp_accumulate_chunk(term, matched, acc64);
-            pending = 0;
-            matched = false;
-        }
-#else
         float term[32];
 #pragma unroll
         for (int k = 0; k < 32; ++k) term[k] = 0.f;
@@ -1453,18 +1262,10 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
         if (i < n)
             matched = icp_process_query<L2LOSS, MODE, COLORED>(a, s_U, i, p, jp, clear_prev, &sl.ts[lane], &sl.ns[lane],
                                                                &sl.cg[COLORED ? lane : 0], term);
-#if ICP_TRANSPOSE_SMEM
-        icp_accumulate_chunk_smem(term, matched, sm.tr[w], acc64);
-#else
         icp_accumulate_chunk(term, matched, acc64);
-#endif
-#endif
     }
-#if ICP_DEFER > 1
-    if (pending) icp_accumulate_chunk(term, matched, acc64);
-#endif
     if (lane < kNumSums) s_warp[w][lane] = acc64;
-    icp_block_epilogue<MODE, kIcpT>(a, s_warp, s_final);
+    icp_block_epilogue<MODE>(a, s_warp, s_final);
 }
 
 // Multi-GPU: runs after the all-reduce of st->sums.
@@ -1494,7 +1295,6 @@ struct o3db_icp {
     double n_total = 0;
     double init_T[16];
     char* src_blk = nullptr;         // chunk-blocked working source: points, seeds, clearances (SrcBlocked)
-    long long* dbg = nullptr;        // ICP_TIMING builds only
     unsigned* src_key = nullptr;     // cell key of every source point (sort order)
     unsigned* src_rank = nullptr;
     unsigned* src_start = nullptr;   // CSR offsets of the source sort
@@ -1504,7 +1304,6 @@ struct o3db_icp {
     IcpState* h_st = nullptr;        // pinned
     o3db_comm* comm = nullptr;
     int grid_blocks = 0;
-    int variant = 2;                 // 1 = direct loads, 2 = staged (TMA + cp.async ring; default)
     int64_t src_keys = 0;            // size of the source sort key space
     int launched = 0;
     bool l2loss = true;
@@ -1519,39 +1318,22 @@ struct o3db_icp {
 namespace o3db {
 
 typedef void (*IcpKernel)(IcpArgs);
-// mode 0 = iterate (loss / colour / variant of the handle), 1 = final evaluation (no Jacobian)
+// mode 0 = iterate (loss / colour of the handle), 1 = final evaluation (no Jacobian)
 static IcpKernel icp_kernel_for(const o3db_icp* c, int mode) {
-    if (c->variant == 1) {
-        if (mode == 1) return icp_iteration_direct_kernel<true, 1, false>;
-        if (c->colored) return c->l2loss ? icp_iteration_direct_kernel<true, 0, true> : icp_iteration_direct_kernel<false, 0, true>;
-        return c->l2loss ? icp_iteration_direct_kernel<true, 0, false> : icp_iteration_direct_kernel<false, 0, false>;
-    }
     if (mode == 1) return icp_iteration_kernel<true, 1, false>;
     if (c->colored) return c->l2loss ? icp_iteration_kernel<true, 0, true> : icp_iteration_kernel<false, 0, true>;
     return c->l2loss ? icp_iteration_kernel<true, 0, false> : icp_iteration_kernel<false, 0, false>;
 }
 
-// Launch with the programmatic-stream-serialization attribute: the kernel's griddepcontrol.wait orders it
-// after the previous kernel on the stream; everything before that wait may overlap the predecessor's tail.
-// dynamic shared memory of the handle's iteration kernels (the staged variant: stage ring + transpose tile)
-static int icp_threads(const o3db_icp* c) { return c->variant == 1 ? kThreads : kIcpT; }
+// dynamic shared memory of the handle's iteration kernels (the stage ring)
 static size_t icp_smem_bytes(const o3db_icp* c, int mode) {
-    if (c->variant == 1) return 0;
     return (c->colored && mode == 0) ? sizeof(IcpStagedSmem<true>) : sizeof(IcpStagedSmem<false>);
 }
 
-static cudaError_t launch_icp(IcpKernel kernel, int blocks, size_t smem, cudaStream_t st, const IcpArgs& a, int threads) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)blocks);
-    cfg.blockDim = dim3((unsigned)threads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = ICP_PDL ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kernel, a);
+// The kernel's griddepcontrol.wait orders it after the previous kernel on the stream; everything before that wait
+// may overlap the predecessor's tail.
+static cudaError_t launch_icp(const o3db_icp* c, int mode, cudaStream_t st, const IcpArgs& a) {
+    return launch_pdl_ex(icp_kernel_for(c, mode), {(unsigned)c->grid_blocks, kIcpThreads, icp_smem_bytes(c, mode)}, st, a);
 }
 static IcpArgs make_args(o3db_icp* c) {
     IcpArgs a{};
@@ -1560,7 +1342,6 @@ static IcpArgs make_args(o3db_icp* c) {
     a.nrm = c->nns.nrm4;
     a.cs = c->nns.cell_start;
     a.src = SrcBlocked{c->src_blk};
-    a.dbg = c->dbg;
     a.n = c->n;
     a.n_total = c->n_total;
     const float r = (float)c->opt.max_correspondence_distance;
@@ -1903,7 +1684,6 @@ void o3db_icp_destroy(o3db_icp* c) {
     cudaStreamSynchronize(st);
     nns_free(&c->nns, st);
     if (c->src_blk) cudaFreeAsync(c->src_blk, st);
-    if (c->dbg) cudaFreeAsync(c->dbg, st);
     if (c->src_key) cudaFreeAsync(c->src_key, st);
     if (c->src_rank) cudaFreeAsync(c->src_rank, st);
     if (c->src_start) cudaFreeAsync(c->src_start, st);
@@ -1980,15 +1760,12 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     } while (0)
     // fitness denominator over all ranks
     c->n_total = (double)n;
-    // 1 = direct (every load where it is needed), 2 = staged (TMA bulk copies + cp.async gathers one chunk
-    // ahead).  Default: staged, 1.6 % faster than direct on an H100 (DESIGN.md §4.1, profiles/h100_icp_ab.jsonl).
-    c->variant = options->search_variant == 1 ? 1 : (options->search_variant == 2 ? 2 : ICP_DEFAULT_VARIANT);
     int occ = 1;
     for (int mode = 0; mode < 2; ++mode)
         ICP_CUDA(cudaFuncSetAttribute(icp_kernel_for(c, mode), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)icp_smem_bytes(c, mode)));
-    ICP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, icp_kernel_for(c, 0), icp_threads(c), icp_smem_bytes(c, 0)));
-    c->grid_blocks = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, icp_threads(c)), (int64_t)num_sms() * std::max(occ, 1)));
+    ICP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, icp_kernel_for(c, 0), kIcpThreads, icp_smem_bytes(c, 0)));
+    c->grid_blocks = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, kIcpThreads), (int64_t)num_sms() * std::max(occ, 1)));
     const int64_t ncell = tiled_key_space(c->nns.g.nx, c->nns.g.ny, c->nns.g.nz);   // tile-major source keys
     c->src_keys = ncell;
     // padded to whole 256-entry chunks: the staged kernel copies 32-entry chunks with TMA bulk copies
@@ -2001,10 +1778,6 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     ICP_CUDA(cudaMallocAsync(&c->src_rank, n * sizeof(unsigned), st));
     ICP_CUDA(cudaMallocAsync(&c->src_start, (ncell + 1) * sizeof(unsigned), st));
     ICP_CUDA(cudaMallocAsync(&c->partials, (size_t)c->grid_blocks * kSumStride * sizeof(double), st));
-#if ICP_TIMING
-    ICP_CUDA(cudaMallocAsync(&c->dbg, (size_t)c->grid_blocks * 8 * sizeof(long long), st));
-    ICP_CUDA(cudaMemsetAsync(c->dbg, 0, (size_t)c->grid_blocks * 8 * sizeof(long long), st));
-#endif
     ICP_CUDA(cudaMallocAsync(&c->per_iter, (size_t)std::max(1, options->max_iteration) * 2 * sizeof(double), st));
     ICP_CUDA(cudaMallocAsync(&c->st, sizeof(IcpState), st));
     static_assert(sizeof(IcpState) <= 4096, "IcpState must fit a pinned block");
@@ -2089,16 +1862,6 @@ int o3db_icp_create_colored(const float* source_dev, const float* source_colors_
     return icp_create_impl(source_dev, n, target_dev, target_normals_dev, m, init_T, options, comm, col, stream, out);
 }
 
-#if ICP_TIMING
-// diagnostics build only: copies the per-block timestamps of the most recent iteration launch (8 per block)
-int o3db_icp_debug_timing(o3db_icp* c, long long* out_host, int max_blocks, int* blocks) {
-    cudaStreamSynchronize(c->stream);
-    const int nb = std::min(max_blocks, c->grid_blocks);
-    if (blocks) *blocks = c->grid_blocks;
-    return cudaMemcpy(out_host, c->dbg, (size_t)nb * 8 * sizeof(long long), cudaMemcpyDeviceToHost) == cudaSuccess ? O3DB_OK : O3DB_ERR_CUDA;
-}
-#endif
-
 int o3db_icp_reset(o3db_icp* c, void* stream) {
     O3DB_REQUIRE(c != nullptr, "o3db_icp_reset: null handle");
     cudaStream_t st = (cudaStream_t)stream;
@@ -2113,7 +1876,7 @@ int o3db_icp_iterate(o3db_icp* c, int iterations, void* stream) {
     const int todo = std::min(iterations, c->opt.max_iteration - c->launched);
     IcpArgs a = make_args(c);
     for (int k = 0; k < todo; ++k) {
-        launch_icp(icp_kernel_for(c, 0), c->grid_blocks, icp_smem_bytes(c, 0), st, a, icp_threads(c));
+        launch_icp(c, 0, st, a);
         O3DB_LAUNCH_CHECK();
         if (!a.fuse_finalize) {
             int rc = o3db_comm_allreduce_f64(c->comm, (double*)((char*)c->st + offsetof(IcpState, sums)), kNumSums, st);
@@ -2160,7 +1923,7 @@ int o3db_icp_finish(o3db_icp* c, o3db_icp_result* result, int64_t* correspondenc
     cudaStream_t st = (cudaStream_t)stream;
     IcpArgs a = make_args(c);
     a.corr_out = correspondences_dev;
-    launch_icp(icp_kernel_for(c, 1), c->grid_blocks, icp_smem_bytes(c, 1), st, a, icp_threads(c));
+    launch_icp(c, 1, st, a);
     O3DB_LAUNCH_CHECK();
     if (!a.fuse_finalize) {
         int rc = o3db_comm_allreduce_f64(c->comm, (double*)((char*)c->st + offsetof(IcpState, sums)), kNumSums, st);

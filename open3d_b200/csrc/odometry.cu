@@ -21,8 +21,6 @@
 #include <chrono>
 #include <climits>
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <new>
@@ -37,9 +35,7 @@
 namespace o3db {
 
 static constexpr int kOT = 256;
-#ifndef ODO_BLOCKS_PER_SM
-#define ODO_BLOCKS_PER_SM 4   // blocks per SM of the iteration kernel; fewer = shorter serial tail in the last block (tunable)
-#endif
+static constexpr int kOdoBlocksPerSm = 4;   // blocks per SM of the iteration kernel; fewer = shorter serial tail in the last block
 
 // ------------------------------------------------------------ image kernels
 
@@ -215,14 +211,13 @@ __device__ __forceinline__ float pyr_down_pixel(const float* __restrict__ img, i
     return den == 0 ? invalid_fill : dvd(num, den);
 }
 
-// kUnrollRows: the 5 x 5 tap loop fully unrolled (64 registers, 4 blocks per SM) or by rows (48 registers, 5 blocks).
-template <bool kUnrollRows>
+// The 5 x 5 tap loop is unrolled by rows only: 48 registers and 5 blocks per SM, against 64 and 4 fully unrolled.
 __global__ void __launch_bounds__(kTW* kTH) pyramid_level_kernel(LevelArgs a) {
     __shared__ float s_depth[kTH + 5][kTW + 5];       // target depth, rows y0-2 .. y0+kTH+2, cols x0-2 .. x0+kTW+2 (clamped)
     __shared__ float s_vert[kTH + 1][kTW + 1][3];     // vertices of the smoothed depth at the normal stencil points
     __shared__ float s_wpos[5][5];                    // the filter's spatial weights: one division + expf each, once per block
-    pdl_grid_wait();
-    pdl_grid_launch_dependents();
+    pdl_wait();
+    pdl_launch_dependents();
     if (a.init_state && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
         // RGBDOdometry.cpp:165 OdometryResult(trans, /*prev rmse*/ 0.0, /*prev fitness*/ 1.0); the iteration kernels read
         // it after their griddepcontrol.wait, i.e. after every pyramid launch has completed
@@ -269,13 +264,8 @@ __global__ void __launch_bounds__(kTW* kTH) pyramid_level_kernel(LevelArgs a) {
                     den = add(den, w);
                 }
             };
-            if constexpr (kUnrollRows) {
-#pragma unroll
-                for (int dy = 0; dy < 5; ++dy) taps_of_row(dy);
-            } else {
 #pragma unroll 1
-                for (int dy = 0; dy < 5; ++dy) taps_of_row(dy);
-            }
+            for (int dy = 0; dy < 5; ++dy) taps_of_row(dy);
             const float smooth = dvd(num, den);
             if (!is_invalid(smooth, a.invalid_fill)) unproject(a.ti, (float)gx, (float)gy, smooth, vx, vy, vz);
         }
@@ -339,8 +329,8 @@ template <typename s_t, typename t_t>
 __global__ void clip_transform_pair_kernel(const s_t* __restrict__ src, const t_t* __restrict__ tgt, int64_t n, float scale,
                                            float min_value, float max_value, float clip_fill, float* __restrict__ src_out,
                                            float* __restrict__ tgt_out) {
-    pdl_grid_wait();
-    pdl_grid_launch_dependents();
+    pdl_wait();
+    pdl_launch_dependents();
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= n) return;
     float out = blockIdx.y == 0 ? dvd((float)src[i], scale) : dvd((float)tgt[i], scale);   // ImageImpl.h:112-116
@@ -521,8 +511,8 @@ __global__ void __launch_bounds__(kThreads) odometry_iteration_kernel(OdoArgs a)
     __shared__ double s_final[kSumStride];
     __shared__ Cam s_cam;
     __shared__ int s_skip;
-    pdl_grid_wait();                 // the previous iteration's T / flags, the pyramid kernels' maps
-    pdl_grid_launch_dependents();
+    pdl_wait();                 // the previous iteration's T / flags, the pyramid kernels' maps
+    pdl_launch_dependents();
     if (threadIdx.x == 0) s_skip = (*(volatile int*)&a.st->level_done[a.level]) | (*(volatile int*)&a.st->status);
     if (threadIdx.x < 12) s_cam.e[threadIdx.x / 4][threadIdx.x % 4] = (float)a.st->T[threadIdx.x];   // TransformIndexer: f32
     if (threadIdx.x == 12) {
@@ -582,9 +572,8 @@ __global__ void __launch_bounds__(kThreads) odometry_iteration_kernel(OdoArgs a)
 static constexpr int kLevelThreads = 512;
 static constexpr int kMaxCluster = 16;
 static constexpr int kLevelFlush = 16;       // f32 terms per thread between two warp reductions (at most kLevelFlush + kLevelBatch - 1)
+static constexpr int kLevelBatch = 3;        // pixels a thread has in flight
 
-// kLevelBatch: pixels a thread has in flight.
-template <int kLevelBatch>
 __global__ void __launch_bounds__(kLevelThreads, 1) odometry_level_kernel(OdoArgs a, int max_iteration) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
@@ -596,8 +585,8 @@ __global__ void __launch_bounds__(kLevelThreads, 1) odometry_level_kernel(OdoArg
     __shared__ OdoState s_st;
     __shared__ Cam s_cam;
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    pdl_grid_wait();                 // the previous level's T / flags, the pyramid kernels' maps
-    pdl_grid_launch_dependents();
+    pdl_wait();                 // the previous level's T / flags, the pyramid kernels' maps
+    pdl_launch_dependents();
     for (int k = threadIdx.x; k < kStateWords; k += kLevelThreads)
         reinterpret_cast<unsigned long long*>(&s_st)[k] = reinterpret_cast<const unsigned long long*>(a.st)[k];
     __syncthreads();
@@ -845,7 +834,7 @@ static void odo_scratch_free(OdoScratch* s, cudaStream_t st, bool pinned_idle = 
 static int odo_scratch_alloc(OdoScratch* s, int64_t pixels, int log_entries, const double* T, cudaStream_t st,
                              bool device_init = false) {
     configure_memory_pool();
-    s->blocks = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(pixels, kThreads), (int64_t)num_sms() * ODO_BLOCKS_PER_SM));
+    s->blocks = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(pixels, kThreads), (int64_t)num_sms() * kOdoBlocksPerSm));
     static_assert(sizeof(OdoState) <= 4096 - 64, "OdoState and the token must fit a pinned block");
     static_assert(kStateWords <= kHostTokenWord && (kHostTokenWord + 1) * sizeof(unsigned long long) <= 4096, "token placement");
     O3DB_CUDA_CHECK(cudaMallocAsync(&s->st, sizeof(OdoState), st));
@@ -882,7 +871,7 @@ static int odo_status_to_rc(int status) {
 
 // Cluster size the level-resident kernel runs with on the current device: 16 CTAs (non-portable size, one GPC) when
 // the device can co-schedule such a cluster, else 8, else 0 = the per-iteration kernel everywhere.  Decided once per
-// device.  O3DB_ODO_LEVEL_CLUSTER = 0 | 8 | 16 caps it (measurements, fallback).
+// device.
 static int level_cluster_size() {
     static std::mutex mu;
     static int cached[64];
@@ -891,14 +880,9 @@ static int level_cluster_size() {
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 0;
     std::lock_guard<std::mutex> lk(mu);
     if (known[dev]) return cached[dev];
-    int cap = 16;
-    if (const char* e = getenv("O3DB_ODO_LEVEL_CLUSTER")) cap = atoi(e);
     int chosen = 0;
     for (int c : {16, 8}) {
-        if (c > cap) continue;
-        if (c > 8 && (cudaFuncSetAttribute(odometry_level_kernel<1>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
-                      cudaFuncSetAttribute(odometry_level_kernel<3>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
-                      cudaFuncSetAttribute(odometry_level_kernel<4>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess)) {
+        if (c > 8 && cudaFuncSetAttribute(odometry_level_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) {
             cudaGetLastError();
             continue;
         }
@@ -913,7 +897,7 @@ static int level_cluster_size() {
         cfg.attrs = attr;
         cfg.numAttrs = 1;
         int clusters = 0;
-        if (cudaOccupancyMaxActiveClusters(&clusters, odometry_level_kernel<4>, &cfg) == cudaSuccess && clusters >= 1) {
+        if (cudaOccupancyMaxActiveClusters(&clusters, odometry_level_kernel, &cfg) == cudaSuccess && clusters >= 1) {
             chosen = c;
             break;
         }
@@ -921,48 +905,12 @@ static int level_cluster_size() {
     }
     cached[dev] = chosen;
     known[dev] = true;
-    if (getenv("O3DB_ODO_VERBOSE")) fprintf(stderr, "[o3db] odometry level-resident kernel: cluster of %d CTAs on device %d\n", chosen, dev);
     return chosen;
 }
 
 // Pixels per thread up to which a level runs in the level-resident kernel: beyond that the cluster's 8 - 16 SMs are
 // slower at the pixel loop than the whole GPU is at the per-iteration kernel's fixed cost.
-static int level_pixels_per_thread() {
-    static const int v = [] {
-        const char* e = getenv("O3DB_ODO_LEVEL_PX_PER_THREAD");
-        return e ? atoi(e) : 12;
-    }();
-    return v;
-}
-
-// O3DB_ODO_NO_ZERO_COPY=1: read the result back with a copy + stream synchronisation (measurements, fallback)
-static bool zero_copy_result() {
-    static const bool v = getenv("O3DB_ODO_NO_ZERO_COPY") == nullptr;
-    return v;
-}
-
-static cudaError_t launch_level(const OdoArgs& a, int max_iteration, int cluster, cudaStream_t st) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)cluster);
-    cfg.blockDim = dim3(kLevelThreads);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    attr[1].id = cudaLaunchAttributeClusterDimension;
-    attr[1].val.clusterDim.x = (unsigned)cluster;
-    attr[1].val.clusterDim.y = 1;
-    attr[1].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 2;
-    static const int batch = [] {       // pixels in flight per thread (O3DB_ODO_LEVEL_BATCH = 1 | 3 | 4: measurements)
-        const char* v = getenv("O3DB_ODO_LEVEL_BATCH");
-        return v ? atoi(v) : 3;
-    }();
-    if (batch <= 1) return cudaLaunchKernelEx(&cfg, odometry_level_kernel<1>, a, max_iteration);
-    if (batch >= 4) return cudaLaunchKernelEx(&cfg, odometry_level_kernel<4>, a, max_iteration);
-    return cudaLaunchKernelEx(&cfg, odometry_level_kernel<3>, a, max_iteration);
-}
+static constexpr int kLevelPixelsPerThread = 12;
 
 }  // namespace o3db
 
@@ -1070,21 +1018,12 @@ int o3db_rgbd_odometry_multi_scale_point_to_plane(const void* source_depth_dev, 
     // RGBDOdometry.cpp:84-88 ClipTransform(depth_scale, 0, depth_max, NAN), both frames in one launch
     if (rc == O3DB_OK) {
         const int64_t npx = (int64_t)rows * cols;
-        const dim3 grid((unsigned)launch_image_1d(npx), 2);
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = grid;
-        cfg.blockDim = dim3(kOT);
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
+        const PdlLaunch shape{dim3((unsigned)launch_image_1d(npx), 2), kOT};
         cudaError_t e;
         const bool su = source_dtype == O3DB_DEPTH_U16, tu = target_dtype == O3DB_DEPTH_U16;
-#define ODO_CLIP(S, T)                                                                                                   \
-    e = cudaLaunchKernelEx(&cfg, clip_transform_pair_kernel<S, T>, (const S*)source_depth_dev, (const T*)target_depth_dev, npx, \
-                           depth_scale, 0.0f, depth_max, nanf_, src_d, tgt_d)
+#define ODO_CLIP(S, T)                                                                                                 \
+    e = launch_pdl_ex(clip_transform_pair_kernel<S, T>, shape, st, source_depth_dev, target_depth_dev, npx, depth_scale, \
+                      0.0f, depth_max, nanf_, src_d, tgt_d)
         if (su && tu) ODO_CLIP(uint16_t, uint16_t);
         else if (su) ODO_CLIP(uint16_t, float);
         else if (tu) ODO_CLIP(float, uint16_t);
@@ -1130,21 +1069,8 @@ int o3db_rgbd_odometry_multi_scale_point_to_plane(const void* source_depth_dev, 
             la.tgt_next = last ? nullptr : smooth;
             la.init_state = i == 0 ? s.st : nullptr;
             for (int k = 0; k < 16; ++k) la.init_T[k] = init_source_to_target[k];
-            cudaLaunchConfig_t cfg{};
-            cfg.gridDim = dim3((unsigned)ceil_div(c, kTW), (unsigned)ceil_div(r, kTH));
-            cfg.blockDim = dim3(kTW * kTH);
-            cfg.stream = st;
-            cudaLaunchAttribute attr[1];
-            attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            attr[0].val.programmaticStreamSerializationAllowed = 1;
-            cfg.attrs = attr;
-            cfg.numAttrs = 1;
-            static const bool unroll_rows = [] {
-                const char* v = getenv("O3DB_ODO_PYR_UNROLL");
-                return v ? atoi(v) != 0 : false;
-            }();
-            const cudaError_t e = unroll_rows ? cudaLaunchKernelEx(&cfg, pyramid_level_kernel<true>, la)
-                                              : cudaLaunchKernelEx(&cfg, pyramid_level_kernel<false>, la);
+            const cudaError_t e = launch_pdl_ex(
+                    pyramid_level_kernel, {dim3((unsigned)ceil_div(c, kTW), (unsigned)ceil_div(r, kTH)), kTW * kTH}, st, la);
             count_launch();
             if (e != cudaSuccess) {
                 set_last_error("pyramid_level_kernel launch failed: %s", cudaGetErrorString(e));
@@ -1167,7 +1093,7 @@ int o3db_rgbd_odometry_multi_scale_point_to_plane(const void* source_depth_dev, 
     static std::atomic<unsigned long long> g_token{0};
     const unsigned long long token = ++g_token;
     volatile unsigned long long* h_words = reinterpret_cast<volatile unsigned long long*>(s.h_st);
-    const bool zero_copy = zero_copy_result() && final_level >= 0 && rc == O3DB_OK;
+    const bool zero_copy = final_level >= 0 && rc == O3DB_OK;
     if (zero_copy) h_words[kHostTokenWord] = 0;
     for (int i = 0; i < num_levels && rc == O3DB_OK; ++i) {
         OdoArgs a{};
@@ -1193,13 +1119,14 @@ int o3db_rgbd_odometry_multi_scale_point_to_plane(const void* source_depth_dev, 
         const int cluster = level_cluster_size();
         cudaError_t e = cudaSuccess;
         if (cluster > 0 && criteria[i].max_iteration >= 2 &&
-            pixels <= (int64_t)cluster * kLevelThreads * level_pixels_per_thread()) {
+            pixels <= (int64_t)cluster * kLevelThreads * kLevelPixelsPerThread) {
             // a coarse level: all its iterations in one launch of one thread-block cluster
             if (zero_copy && i == final_level) {
                 a.host_out = const_cast<unsigned long long*>(h_words);
                 a.host_token = token;
             }
-            e = launch_level(a, criteria[i].max_iteration, cluster, st);
+            e = launch_pdl_ex(odometry_level_kernel, {(unsigned)cluster, kLevelThreads, 0, (unsigned)cluster}, st, a,
+                              criteria[i].max_iteration);
             count_launch();
         } else {
             for (int it = 0; it < criteria[i].max_iteration && e == cudaSuccess; ++it) {
@@ -1207,7 +1134,7 @@ int o3db_rgbd_odometry_multi_scale_point_to_plane(const void* source_depth_dev, 
                     a.host_out = const_cast<unsigned long long*>(h_words);
                     a.host_token = token;
                 }
-                e = launch_pdl_ex(odometry_iteration_kernel, (unsigned)blocks, (unsigned)kThreads, 0, st, a);
+                e = launch_pdl_ex(odometry_iteration_kernel, {(unsigned)blocks, kThreads}, st, a);
                 count_launch();
             }
         }

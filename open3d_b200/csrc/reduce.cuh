@@ -11,10 +11,7 @@ namespace o3db {
 static constexpr int kThreads = 256;
 static constexpr int kNumSums = 30;   // 29 reference slots + sum of dist^2
 static constexpr int kSumStride = 32;
-#ifndef ICP_FLUSH_EVERY
-#define ICP_FLUSH_EVERY 32
-#endif
-static constexpr int kFlushEvery = ICP_FLUSH_EVERY;   // f32 terms per thread before the f64 tree (error <= kFlushEvery * 2^-24 of sum|term|)
+static constexpr int kFlushEvery = 32;   // f32 terms per thread before the f64 tree (error <= kFlushEvery * 2^-24 of sum|term|)
 
 // ------------------------------------------------- 29(+1)-scalar reduction
 
@@ -51,40 +48,25 @@ __device__ __forceinline__ float warp_transpose_sum32(float (&v)[32]) {
     return v[0];
 }
 
-#ifndef O3DB_FENCE_ACQREL
-#define O3DB_FENCE_ACQREL 0
-#endif
-// release of the block partial before the ticket / acquire of everybody's partials after it
-__device__ __forceinline__ void reduce_fence() {
-#if O3DB_FENCE_ACQREL
-    asm volatile("fence.acq_rel.gpu;" ::: "memory");
-#else
-    __threadfence();
-#endif
-}
-
 // Block epilogue: per-warp slots -> block partial -> (last block) grand total in
 // block-index order.  Returns true in the last block, with s_final[] filled.
 template <int THREADS = kThreads>
 __device__ __forceinline__ bool block_reduce_to_global(double (*s_warp)[kSumStride], double* __restrict__ partials,
-                                                       unsigned* ticket, double* s_final,
-                                                       long long* stamps = nullptr) {
+                                                       unsigned* ticket, double* s_final) {
     __shared__ bool s_last;
     __syncthreads();
-    if (stamps && threadIdx.x == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(stamps[0]));
     if (threadIdx.x < kNumSums) {
         double v = 0;
 #pragma unroll
         for (int w = 0; w < THREADS / 32; ++w) v += s_warp[w][threadIdx.x];
         partials[(size_t)blockIdx.x * kSumStride + threadIdx.x] = v;
     }
-    reduce_fence();
+    __threadfence();   // release of the block partial before the ticket
     __syncthreads();
     if (threadIdx.x == 0) s_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
     __syncthreads();
     if (!s_last) return false;
-    if (stamps && threadIdx.x == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(stamps[1]));
-    reduce_fence();
+    __threadfence();   // acquire of everybody's partials after it
     // Grand total by the WHOLE block (round 1 had 30 threads walk all per-block partials one dependent
     // L2 round trip at a time: ~130k cycles for 444 blocks, a third of the kernel): warp w sums the blocks
     // b = w, w + 8, ... for all 30 columns (lane = column, 256-byte coalesced rows, 8 loads in flight),

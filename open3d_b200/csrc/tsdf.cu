@@ -31,38 +31,16 @@ static constexpr int kSamples = kStepSize + 1;      // est_multipler_factor
 static constexpr int kStride = 4;                   // VoxelBlockGrid.cpp:221 down_factor
 static constexpr int kPinnedInts = 16 + 8 * 16;     // o3db_vbg::h_pinned: [0..15] synchronous read-back, then a ring of 8 x 16
 
-// Programmatic dependent launch (both frame kernels are launched with the attribute): the grid may become
-// resident while its predecessor on the stream drains; nothing the predecessor wrote is read before the wait.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-__device__ __forceinline__ unsigned smem_addr(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* b, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(b)), "r"(count) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive(unsigned long long* b) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(b)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long* b, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* b, unsigned parity) {
-    unsigned done;
-    do {
-        asm volatile(
-                "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                : "=r"(done)
-                : "r"(smem_addr(b)), "r"(parity)
-                : "memory");
-    } while (!done);
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory");
 }
 // 2-D tiled TMA load (cp.async.bulk.tensor, SASS UTMALDG): box of the descriptor at element (x, y) of the image;
 // out-of-image elements are zero-filled by the copy engine, completion is signalled on the mbarrier.
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int x, int y, unsigned long long* b) {
     asm volatile(
             "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-                    smem_addr(dst)),
-            "l"(map), "r"(smem_addr(b)), "r"(x), "r"(y)
+                    smem_u32(dst)),
+            "l"(map), "r"(smem_u32(b)), "r"(x), "r"(y)
             : "memory");
 }
 
@@ -592,11 +570,7 @@ __global__ void __launch_bounds__(kT) integrate16_kernel(const __grid_constant__
     }
     pdl_wait();                 // the touch kernel's lists / counters, the previous frame's size
     pdl_launch_dependents();
-    if (a.exec_ns && tid == 0) {
-        unsigned long long now;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-        atomicMin(&a.exec_ns[0], now);
-    }
+    if (a.exec_ns && tid == 0) atomicMin(&a.exec_ns[0], (unsigned long long)global_ns());
     const bool fused = a.counters != nullptr;
     int n_exist = 0, n_new = 0, n_total = a.n_blocks, size0 = 0;
     bool drop = false;
@@ -839,8 +813,7 @@ __global__ void __launch_bounds__(kT) integrate16_kernel(const __grid_constant__
             a.counters[3] = 0;
             if (a.work) *a.work = 0;
             if (a.exec_ns) {
-                unsigned long long now;
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+                const unsigned long long now = global_ns();
                 a.exec_ns[1] += now - a.exec_ns[0];
                 a.exec_ns[2] += 1;
                 a.exec_ns[0] = ~0ull;
@@ -940,23 +913,6 @@ static const float* inv_weight_table() {
         tab[dev] = p;
     }
     return tab[dev];
-}
-
-// Launch with the programmatic-stream-serialization attribute (the kernels call griddepcontrol.wait before they
-// touch anything a predecessor wrote).
-template <typename... KArgs, typename... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), unsigned grid, cudaStream_t st, Args&&... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kT);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
 static unsigned pow2_at_least(int64_t v) {
@@ -1067,12 +1023,11 @@ static int launch_integrate_typed(o3db_vbg* v, IntegrateArgs& a, int depth_dtype
     cudaError_t e;
     if (v->resolution == 16 && a.rows <= 32767 && a.cols <= 65535) {
         CUtensorMap map;
-        static const bool no_tile = getenv("O3DB_TSDF_NO_TILE") != nullptr;   // A/B knob: read the depth image directly
-        a.use_tile = (!no_tile && make_depth_tensor_map(&map, a.depth, depth_dtype, a.rows, a.cols)) ? 1 : 0;
+        a.use_tile = make_depth_tensor_map(&map, a.depth, depth_dtype, a.rows, a.cols) ? 1 : 0;
         if (!a.use_tile) memset(&map, 0, sizeof(map));
-        e = launch_pdl(integrate16_kernel<depth_t, color_in_t, HAS_COLOR>, grid, st, a, map);
+        e = launch_pdl_ex(integrate16_kernel<depth_t, color_in_t, HAS_COLOR>, {grid, kT}, st, a, map);
     } else {
-        e = launch_pdl(integrate_kernel<depth_t, color_in_t, HAS_COLOR>, grid, st, a);
+        e = launch_pdl_ex(integrate_kernel<depth_t, color_in_t, HAS_COLOR>, {grid, kT}, st, a);
     }
     count_launch();
     if (e != cudaSuccess) {
@@ -1552,11 +1507,11 @@ int o3db_integrate_blocks(const void* depth_dev, int depth_dtype, const void* co
     const unsigned grid = (unsigned)std::min<int64_t>(num_blocks, (int64_t)num_sms() * 8);
     cudaError_t e = cudaErrorInvalidValue;
     if (depth_dtype == O3DB_DEPTH_U16 && (!has_color || color_dtype == O3DB_COLOR_U8)) {
-        e = has_color ? launch_pdl(integrate_kernel<uint16_t, uint8_t, true, float, float>, grid, st, a)
-                      : launch_pdl(integrate_kernel<uint16_t, uint8_t, false, float, float>, grid, st, a);
+        e = has_color ? launch_pdl_ex(integrate_kernel<uint16_t, uint8_t, true, float, float>, {grid, kT}, st, a)
+                      : launch_pdl_ex(integrate_kernel<uint16_t, uint8_t, false, float, float>, {grid, kT}, st, a);
     } else if (depth_dtype == O3DB_DEPTH_F32 && (!has_color || color_dtype == O3DB_COLOR_F32)) {
-        e = has_color ? launch_pdl(integrate_kernel<float, float, true, float, float>, grid, st, a)
-                      : launch_pdl(integrate_kernel<float, float, false, float, float>, grid, st, a);
+        e = has_color ? launch_pdl_ex(integrate_kernel<float, float, true, float, float>, {grid, kT}, st, a)
+                      : launch_pdl_ex(integrate_kernel<float, float, false, float, float>, {grid, kT}, st, a);
     } else {
         set_last_error("Unsupported input data type combination. Expected (float, float) or (uint16, uint8)");
         return O3DB_ERR_INVALID;
@@ -1623,8 +1578,8 @@ int o3db_vbg_integrate_frame(o3db_vbg* v, const void* depth_dev, int depth_dtype
         t.tab = Table{v->table, v->nbuckets - 1, v->keys};
         t.stamp = v->stamp;
         t.frame_id = v->frame_id;
-        const cudaError_t e = depth_dtype == O3DB_DEPTH_U16 ? launch_pdl(touch_kernel<uint16_t>, nb, st, t)
-                                                            : launch_pdl(touch_kernel<float>, nb, st, t);
+        const cudaError_t e = depth_dtype == O3DB_DEPTH_U16 ? launch_pdl_ex(touch_kernel<uint16_t>, {nb, kT}, st, t)
+                                                            : launch_pdl_ex(touch_kernel<float>, {nb, kT}, st, t);
         count_launch();
         if (e != cudaSuccess) {
             set_last_error("touch kernel launch failed: %s", cudaGetErrorString(e));
@@ -1632,11 +1587,6 @@ int o3db_vbg_integrate_frame(o3db_vbg* v, const void* depth_dev, int depth_dtype
         }
         return O3DB_OK;
     };
-    static const bool host_only = getenv("O3DB_TSDF_HOST_ONLY") != nullptr;   // diagnostics: everything but the launches
-    if (host_only) {
-        v->frames += 1;
-        return O3DB_OK;
-    }
     rc = touch();
     if (rc) return rc;
     if (v->frames == 0 || v->sync_next_frame) {

@@ -220,7 +220,6 @@ def _options(max_correspondence_distance, criteria, kernel):
     o.relative_rmse = float(criteria.relative_rmse)
     o.kernel = kernel._c()
     o.cell_scale = 0.0
-    o.search_variant = 0
     return o
 
 
