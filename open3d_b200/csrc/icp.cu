@@ -863,7 +863,7 @@ __device__ void set_identity(double* T, float* Uf) {
 // Threads per block of the iteration kernel: ONE fat block of 24 warps per SM (80 registers x 768 threads fills the
 // register file): a third of the per-block partial rows for the last block to add up (one per SM instead of three)
 // and a third of the block prologues / epilogues; the loop itself has no block-wide barrier either way.  On an H100
-// it is faster than 256 or 512 (profiles/h100_icp_ab.jsonl).
+// it is 3-6 % faster than three 256-thread blocks per SM (profiles/h100_reduce_ab.jsonl).
 static constexpr int kIcpThreads = 768;
 
 // Host part of DoSingleScaleICPIterations (Registration.cpp:293-358), on device, run by ONE WARP once per

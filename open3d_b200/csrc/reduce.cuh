@@ -4,6 +4,8 @@
 // pose -> transformation that the reference runs on the host (kernel/TransformationConverter.cpp).
 #pragma once
 
+#include <utility>
+
 #include "common.cuh"
 
 namespace o3db {
@@ -33,18 +35,22 @@ __device__ __forceinline__ void flush_acc(float (&acc)[kNumSums], double (*s_war
 // (16 + 8 + 4 + 2 + 1 = 31 shuffles for 32 slots) instead of five, and the running totals of a warp live in
 // ONE register per lane instead of 30: the search keeps the register file.  The association is a fixed
 // binary tree over the lanes: deterministic.
+// Every index into v[] is a template argument, not a loop counter, so the array stays in registers whatever the
+// unroller decides.  Written as nested loops over `half`, the sm_90a build kept v[] (and the callers' term arrays) in
+// local memory: 176 B of stack per thread, stored and reloaded through L1 / L2 for every 32-query chunk, which made the
+// ICP iteration 3.3x slower on an H100 (tests/test_local_memory.py guards against it).
+template <int HALF, int... K>
+__device__ __forceinline__ void warp_transpose_step(float (&v)[32], bool up, std::integer_sequence<int, K...>) {
+    ((v[K] = (up ? v[K + HALF] : v[K]) + __shfl_xor_sync(0xffffffffu, up ? v[K] : v[K + HALF], HALF)), ...);
+}
+template <int HALF>
+__device__ __forceinline__ void warp_transpose_steps(float (&v)[32], unsigned lane) {
+    // step HALF: lane keeps v[k + HALF] (upper lane) or v[k] (lower lane) and adds what lane ^ HALF sends, k < HALF
+    warp_transpose_step<HALF>(v, (lane & HALF) != 0, std::make_integer_sequence<int, HALF>{});
+    if constexpr (HALF > 1) warp_transpose_steps<HALF / 2>(v, lane);
+}
 __device__ __forceinline__ float warp_transpose_sum32(float (&v)[32]) {
-    const unsigned lane = threadIdx.x & 31u;
-#pragma unroll
-    for (int half = 16; half >= 1; half >>= 1) {
-        const bool up = (lane & half) != 0;
-#pragma unroll
-        for (int k = 0; k < half; ++k) {
-            const float keep = up ? v[k + half] : v[k];
-            const float send = up ? v[k] : v[k + half];
-            v[k] = keep + __shfl_xor_sync(0xffffffffu, send, half);
-        }
-    }
+    warp_transpose_steps<16>(v, threadIdx.x & 31u);
     return v[0];
 }
 
