@@ -143,18 +143,24 @@ static int canonical_ranks(int64_t n, const unsigned* start, const unsigned* key
     return O3DB_OK;
 }
 
-// Working source, CHUNK-BLOCKED: chunk c (32 consecutive sorted positions) is one 768-byte record
-//   [32 x float4 point (.w = original index) | 32 x int seed | 32 x float clearance]
+// Working source, CHUNK-BLOCKED: chunk c (32 consecutive sorted positions) is one 640-byte record of planes
+//   [32 x float x | 32 x float y | 32 x float z | 32 x int seed | 32 x float clearance]
 // so that everything a warp needs to start a chunk arrives with ONE bulk copy (it took three with separate arrays: 44
-// issue slots per chunk, DESIGN.md 4.1).  24 B per point, as before.
-static constexpr int kSrcChunkBytes = 32 * 16 + 32 * 4 + 32 * 4;
+// issue slots per chunk, DESIGN.md 4.1), and a warp stores a plane back with one coalesced store of at most 128 bytes.
+// 20 B per point.
+// The original index of a sorted position is not in the record: only the evaluation pass (correspondences) and the
+// ColoredICP set-up read it, so it lives in a separate array (o3db_icp::src_idx) that the iterations never move.
+static constexpr int kSrcChunkBytes = 5 * 32 * 4;
 struct SrcBlocked {
     char* base;
     __host__ __device__ static size_t bytes(int64_t n_pad) { return (size_t)(n_pad / 32) * kSrcChunkBytes; }
     __device__ __forceinline__ char* chunk(int i) const { return base + (size_t)(i >> 5) * kSrcChunkBytes; }
-    __device__ __forceinline__ float4* point(int i) const { return reinterpret_cast<float4*>(chunk(i)) + (i & 31); }
-    __device__ __forceinline__ int* seed(int i) const { return reinterpret_cast<int*>(chunk(i) + 512) + (i & 31); }
-    __device__ __forceinline__ float* clearance(int i) const { return reinterpret_cast<float*>(chunk(i) + 640) + (i & 31); }
+    // coordinate `axis` (0 = x, 1 = y, 2 = z) of point i
+    __device__ __forceinline__ float* coord(int axis, int i) const {
+        return reinterpret_cast<float*>(chunk(i) + 128 * axis) + (i & 31);
+    }
+    __device__ __forceinline__ int* seed(int i) const { return reinterpret_cast<int*>(chunk(i) + 384) + (i & 31); }
+    __device__ __forceinline__ float* clearance(int i) const { return reinterpret_cast<float*>(chunk(i) + 512) + (i & 31); }
 };
 
 // no seeds, no clearances (and zeroed padding points)
@@ -163,18 +169,24 @@ __global__ void src_blocked_init_kernel(SrcBlocked sb, int64_t n, int64_t n_pad,
     if (i >= n_pad) return;
     *sb.seed((int)i) = -1;
     *sb.clearance((int)i) = 0.f;
-    if (clear_points && i >= n) *sb.point((int)i) = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (clear_points && i >= n)
+        for (int axis = 0; axis < 3; ++axis) *sb.coord(axis, (int)i) = 0.f;
 }
 
-// scatter of the caller's source into the blocked working copy (clone + initial transform)
+// scatter of the caller's source into the blocked working copy (clone + initial transform); src_idx[sorted position]
+// receives the original index
 __global__ void scatter_source_kernel(const float* __restrict__ pts, int64_t n, Affine T, const unsigned* __restrict__ start,
-                                      const unsigned* __restrict__ key, const unsigned* __restrict__ rank, SrcBlocked sb) {
+                                      const unsigned* __restrict__ key, const unsigned* __restrict__ rank, SrcBlocked sb,
+                                      int* __restrict__ src_idx) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= n) return;
     float x = pts[3 * i], y = pts[3 * i + 1], z = pts[3 * i + 2];
     apply_transform(T.m, x, y, z);
     const unsigned p = start[key[i]] + rank[i];
-    *sb.point((int)p) = make_float4(x, y, z, __int_as_float((int)i));
+    *sb.coord(0, (int)p) = x;
+    *sb.coord(1, (int)p) = y;
+    *sb.coord(2, (int)p) = z;
+    src_idx[p] = (int)i;
 }
 
 template <bool TRANSFORM>
@@ -790,7 +802,8 @@ __global__ void transform_normals_kernel(float* __restrict__ p, int64_t n, Affin
     p[3 * i + 2] = T.m[8] * x + T.m[9] * y + T.m[10] * z;
 }
 
-// ColoredICP side arrays, in the sort order of the working clouds (orig index = .w of the float4)
+// ColoredICP side arrays, in the sort order of the working clouds (orig index = .w of the target's float4, src_idx of
+// the source)
 __global__ void pack_target_color_kernel(const float4* __restrict__ pts4, const float* __restrict__ col,
                                          const float* __restrict__ grad, int64_t m, float4* __restrict__ tcg) {
     const int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -799,11 +812,11 @@ __global__ void pack_target_color_kernel(const float4* __restrict__ pts4, const 
     tcg[j] = make_float4(grad[o], grad[o + 1], grad[o + 2], color_intensity(col[o], col[o + 1], col[o + 2]));
 }
 
-__global__ void pack_source_intensity_kernel(SrcBlocked sb, const float* __restrict__ col,
+__global__ void pack_source_intensity_kernel(const int* __restrict__ src_idx, const float* __restrict__ col,
                                              int64_t n, float* __restrict__ sint) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const int64_t o = 3 * (int64_t)__float_as_int(sb.point((int)i)->w);
+    const int64_t o = 3 * (int64_t)src_idx[i];
     sint[i] = color_intensity(col[o], col[o + 1], col[o + 2]);
 }
 
@@ -828,9 +841,10 @@ struct IcpArgs {
     const float4* tgt;
     const float4* nrm;
     const unsigned* cs;
-    SrcBlocked src;       // working source, sorted, chunk-blocked: point (.w = original index bits), seed = sorted target
-                          // position of its last winner (-1 = none), clearance of that winner (lower bound on the distance
-                          // to every OTHER target point, minus the motion since it was established; 0 = unknown)
+    SrcBlocked src;       // working source, sorted, chunk-blocked: point, seed = sorted target position of its last
+                          // winner (-1 = none), clearance of that winner (lower bound on the distance to every OTHER
+                          // target point, minus the motion since it was established; 0 = unknown)
+    const int* src_idx;   // sorted source position -> original index (read in evaluate mode with corr_out only)
     int64_t n;            // local source points
     double n_total;       // source points over all ranks (fitness denominator)
     float rr, thr;
@@ -979,12 +993,18 @@ __device__ void icp_finalize_evaluate(const IcpArgs& a, const double* sums) {
 // its colour row, fetched by the caller), Jacobian + 30 partial sums, new seed.
 // MODE 0 = iterate, MODE 1 = evaluate (no Jacobian; writes correspondences in the caller's order).
 template <bool L2LOSS, int MODE, bool COLORED>
-__device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float* s_U, int i, float4 p, int jp,
-                                                  float clear_prev, const float4* seed_ts, const float4* seed_nn,
+__device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float* s_U, int i, float px, float py, float pz,
+                                                  int jp, float clear_prev, const float4* seed_ts, const float4* seed_nn,
                                                   const float4* seed_cg, float (&acc)[32]) {
-    const float ox = p.x, oy = p.y, oz = p.z;
-    apply_transform(s_U, p.x, p.y, p.z);
-    *a.src.point(i) = p;
+    const float ox = px, oy = py, oz = pz;
+    apply_transform(s_U, px, py, pz);
+    // Only values whose bits changed are stored back: a store marks its 32-byte sector dirty, and the sector goes back
+    // to HBM, even when it rewrites the bits already there.  Once the clouds are aligned, the pending update leaves
+    // most coordinates (and with them the clearance) bit-for-bit where they were, and a sector of a plane (8 lanes)
+    // whose lanes all skip their store stays clean.
+    if (__float_as_uint(px) != __float_as_uint(ox)) *a.src.coord(0, i) = px;
+    if (__float_as_uint(py) != __float_as_uint(oy)) *a.src.coord(1, i) = py;
+    if (__float_as_uint(pz) != __float_as_uint(oz)) *a.src.coord(2, i) = pz;
     unsigned bj = kNoPoint;
     bool handled = false;
     float clear_new = 0.f;      // what is known about the distance to every point other than the winner
@@ -997,8 +1017,8 @@ __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float*
         // closer than that bound, it is the exact nearest neighbour — no table lookup, no candidate scan.
         // All roundings go against the certificate (round-down subtraction, 1e-5 margins on both roots).
         ts = *seed_ts;
-        const float sd = dist2_canonical(ts, p.x, p.y, p.z);
-        const float mx = p.x - ox, my = p.y - oy, mz = p.z - oz;
+        const float sd = dist2_canonical(ts, px, py, pz);
+        const float mx = px - ox, my = py - oy, mz = pz - oz;
         const float m2 = fmaf(mz, mz, fmaf(my, my, mx * mx));
         const float moved = m2 > 0.f ? __fmul_ru(m2 * rsqrtf(m2), 1.00001f) : 0.f;
         const float clear = __fsub_rd(clear_prev, moved);
@@ -1009,20 +1029,20 @@ __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float*
                 clear_new = clear;
                 handled = true;
             } else {
-                bj = nn_search_seeded_fast(a.g, a.tgt, a.cs, p.x, p.y, p.z, a.rr, a.thr, sd, handled, clear_new);
+                bj = nn_search_seeded_fast(a.g, a.tgt, a.cs, px, py, pz, a.rr, a.thr, sd, handled, clear_new);
             }
         }
     }
     if (!handled) {
-        bj = nn_search_slow(&a.g, a.tgt, a.cs, p.x, p.y, p.z, a.r1, a.r1_accept2, a.rr, a.thr, jp);
+        bj = nn_search_slow(&a.g, a.tgt, a.cs, px, py, pz, a.r1, a.r1_accept2, a.rr, a.thr, jp);
         clear_new = 0.f;
     }
     if ((int)bj != jp) *a.src.seed(i) = (int)bj;
-    *a.src.clearance(i) = clear_new;
+    if (__float_as_uint(clear_new) != __float_as_uint(clear_prev)) *a.src.clearance(i) = clear_new;
     int widx = -1;
     if (bj != kNoPoint) {
         const float4 t = (int)bj == jp ? ts : __ldg(&a.tgt[bj]);   // (just scanned: an L1 hit)
-        const float d = dist2_canonical(t, p.x, p.y, p.z);   // the same arithmetic as inside the scan: same bits
+        const float d = dist2_canonical(t, px, py, pz);   // the same arithmetic as inside the scan: same bits
         widx = __float_as_int(t.w);
         if (MODE == 0) {
             // the seed's normal / colour row were fetched ahead (the winner rarely changes once the clouds
@@ -1030,18 +1050,18 @@ __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float*
             const float4 nn = (int)bj == jp ? *seed_nn : __ldg(&a.nrm[bj]);
             if (COLORED) {
                 const float4 cg = (int)bj == jp ? *seed_cg : __ldg(&a.tcg[bj]);
-                const float vs[3] = {p.x, p.y, p.z}, vt[3] = {t.x, t.y, t.z}, nt[3] = {nn.x, nn.y, nn.z};
+                const float vs[3] = {px, py, pz}, vt[3] = {t.x, t.y, t.z}, nt[3] = {nn.x, nn.y, nn.z};
                 const float dit[3] = {cg.x, cg.y, cg.z};
                 accumulate_colored<L2LOSS, 32>(acc, a.rk, vs, vt, nt, __ldg(&a.sint[i]), cg.w, dit, a.sqrt_lg, a.sqrt_lp);
             } else {
-                accumulate_p2plane<L2LOSS, 32>(acc, a.rk, p.x, p.y, p.z, t.x, t.y, t.z, nn.x, nn.y, nn.z);
+                accumulate_p2plane<L2LOSS, 32>(acc, a.rk, px, py, pz, t.x, t.y, t.z, nn.x, nn.y, nn.z);
             }
         } else {
             acc[28] += 1.0f;
         }
         acc[29] += d;
     }
-    if (MODE == 1 && a.corr_out) a.corr_out[__float_as_int(p.w)] = (int64_t)widx;
+    if (MODE == 1 && a.corr_out) a.corr_out[a.src_idx[i]] = (int64_t)widx;
     return bj != kNoPoint;
 }
 
@@ -1148,9 +1168,8 @@ __device__ __forceinline__ void icp_block_epilogue(const IcpArgs& a, double (*s_
 
 // Per warp, a two-slot ring in shared memory holds what a 32-query chunk needs before its search can
 // start, fetched while the PREVIOUS chunk is being searched:
-//   A  the chunk's source points and seeds: two TMA bulk copies (cp.async.bulk, completion on the slot's
-//      mbarrier) issued by lane 0 two chunks ahead — 512 B + 128 B, contiguous because the working source
-//      is stored sorted;
+//   A  the chunk's record of the working source (points, seeds, clearances): one TMA bulk copy
+//      (cp.async.bulk, completion on the slot's mbarrier) of 640 B issued by lane 0 two chunks ahead;
 //   B  the seeds' target points, normals (and colour rows): one 16-byte cp.async gather per lane and
 //      array, issued one chunk ahead as soon as A has landed (the gather address IS the seed).
 // A query therefore starts with p, seed, seed point and seed normal already on chip, and its dependent
@@ -1159,8 +1178,10 @@ __device__ __forceinline__ void icp_block_epilogue(const IcpArgs& a, double (*s_
 // hands a consumed slot back), accumulator flushes are warp-local.
 template <bool COLORED>
 struct __align__(16) IcpStage {
-    // A: one chunk record of the working source (SrcBlocked): 768 contiguous bytes, ONE bulk copy
-    float4 p[32];      // working source points
+    // A: one chunk record of the working source (SrcBlocked): 640 contiguous bytes, ONE bulk copy
+    float px[32];      // working source points, one plane per coordinate
+    float py[32];
+    float pz[32];
     int jp[32];        // seeds
     float d2[32];      // clearances
     // B: gathered per lane from the seeds
@@ -1215,13 +1236,15 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     const int stride = gridDim.x * kIcpThreads;
     const int first = blockIdx.x * kIcpThreads + w * 32;
     constexpr unsigned kBytesA = kSrcChunkBytes;
-    static_assert(offsetof(IcpStage<COLORED>, jp) == 512 && offsetof(IcpStage<COLORED>, d2) == 640, "stage A mirrors a chunk record");
+    static_assert(offsetof(IcpStage<COLORED>, py) == 128 && offsetof(IcpStage<COLORED>, pz) == 256 &&
+                  offsetof(IcpStage<COLORED>, jp) == 384 && offsetof(IcpStage<COLORED>, d2) == 512 &&
+                  offsetof(IcpStage<COLORED>, ts) == kBytesA, "stage A mirrors a chunk record");
     auto issue_a = [&](int c, int q0) {        // lane 0: ONE TMA bulk copy of chunk c's record into slot c & 1
         if (lane == 0 && q0 < n) {
             IcpStage<COLORED>& sl = sm.stage[w][c & 1];
             unsigned long long* mb = &s_mbar[w][c & 1];
             mbar_arrive_expect_tx(mb, kBytesA);
-            bulk_g2s(sl.p, a.src.chunk(q0), kBytesA, mb);
+            bulk_g2s(sl.px, a.src.chunk(q0), kBytesA, mb);
         }
     };
     auto issue_b = [&](int c, int q0) {        // every lane: gather its seed's rows of chunk c (needs A(c))
@@ -1247,10 +1270,10 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
         IcpStage<COLORED>& sl = sm.stage[w][c & 1];
         // A(c) has landed: every lane waited on its mbarrier in issue_b(c), one trip ago (or in the prologue)
         cp_async_wait_all();                                       // B(c)
-        const float4 p = sl.p[lane];
+        const float px = sl.px[lane], py = sl.py[lane], pz = sl.pz[lane];
         const int jp = sl.jp[lane];
         const float clear_prev = sl.d2[lane];
-        __syncwarp();          // every lane has read p / jp / d2 of slot c & 1: hand that part back to the producer
+        __syncwarp();          // every lane has read its point / jp / d2 of slot c & 1: hand that part back to the producer
         issue_a(c + 2, q0 + 2 * stride);
         issue_b(c + 1, q0 + stride);
         // (ts / ns / cg of slot c & 1 are rewritten by issue_b(c + 2), i.e. in the NEXT trip: still valid below)
@@ -1260,8 +1283,8 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
         for (int k = 0; k < 32; ++k) term[k] = 0.f;
         bool matched = false;
         if (i < n)
-            matched = icp_process_query<L2LOSS, MODE, COLORED>(a, s_U, i, p, jp, clear_prev, &sl.ts[lane], &sl.ns[lane],
-                                                               &sl.cg[COLORED ? lane : 0], term);
+            matched = icp_process_query<L2LOSS, MODE, COLORED>(a, s_U, i, px, py, pz, jp, clear_prev, &sl.ts[lane],
+                                                               &sl.ns[lane], &sl.cg[COLORED ? lane : 0], term);
         icp_accumulate_chunk(term, matched, acc64);
     }
     if (lane < kNumSums) s_warp[w][lane] = acc64;
@@ -1291,10 +1314,11 @@ struct o3db_icp {
     cudaStream_t stream = 0;         // creation stream: allocations are freed on it (o3db_icp_destroy)
     const float* src_user = nullptr;
     int64_t n = 0;
-    int64_t n_pad = 0;               // n rounded up to whole 256-entry chunks (allocation size of src4 / prev)
+    int64_t n_pad = 0;               // n rounded up to whole 256-entry chunks (allocation size of src_blk / src_idx)
     double n_total = 0;
     double init_T[16];
     char* src_blk = nullptr;         // chunk-blocked working source: points, seeds, clearances (SrcBlocked)
+    int* src_idx = nullptr;          // sorted source position -> original index
     unsigned* src_key = nullptr;     // cell key of every source point (sort order)
     unsigned* src_rank = nullptr;
     unsigned* src_start = nullptr;   // CSR offsets of the source sort
@@ -1342,6 +1366,7 @@ static IcpArgs make_args(o3db_icp* c) {
     a.nrm = c->nns.nrm4;
     a.cs = c->nns.cell_start;
     a.src = SrcBlocked{c->src_blk};
+    a.src_idx = c->src_idx;
     a.n = c->n;
     a.n_total = c->n_total;
     const float r = (float)c->opt.max_correspondence_distance;
@@ -1391,7 +1416,8 @@ static int icp_gather_source(o3db_icp* c, cudaStream_t st) {
     for (int i = 0; i < 16; ++i) T0.m[i] = (float)c->init_T[i];   // Transform.cpp:29-31: T cast to the point dtype
     if (c->n == 0) return O3DB_OK;
     scatter_source_kernel<<<(unsigned)ceil_div(c->n, kThreads), kThreads, 0, st>>>(c->src_user, c->n, T0, c->src_start,
-                                                                                  c->src_key, c->src_rank, SrcBlocked{c->src_blk});
+                                                                                  c->src_key, c->src_rank, SrcBlocked{c->src_blk},
+                                                                                  c->src_idx);
     O3DB_LAUNCH_CHECK();
     return O3DB_OK;
 }
@@ -1684,6 +1710,7 @@ void o3db_icp_destroy(o3db_icp* c) {
     cudaStreamSynchronize(st);
     nns_free(&c->nns, st);
     if (c->src_blk) cudaFreeAsync(c->src_blk, st);
+    if (c->src_idx) cudaFreeAsync(c->src_idx, st);
     if (c->src_key) cudaFreeAsync(c->src_key, st);
     if (c->src_rank) cudaFreeAsync(c->src_rank, st);
     if (c->src_start) cudaFreeAsync(c->src_start, st);
@@ -1771,6 +1798,7 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     // padded to whole 256-entry chunks: the staged kernel copies 32-entry chunks with TMA bulk copies
     c->n_pad = ceil_div(n, 256) * 256;
     ICP_CUDA(cudaMallocAsync(&c->src_blk, SrcBlocked::bytes(c->n_pad), st));
+    ICP_CUDA(cudaMallocAsync(&c->src_idx, c->n_pad * sizeof(int), st));
     src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlocked{c->src_blk}, n, c->n_pad, true);
     count_launch();
     ICP_CUDA(cudaGetLastError());
@@ -1813,7 +1841,7 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
         count_launch();
         ICP_CUDA(cudaGetLastError());
         // the source sort order is fixed at creation (o3db_icp_reset re-gathers into the same slots)
-        pack_source_intensity_kernel<<<(unsigned)ceil_div(n, kThreads), kThreads, 0, st>>>(SrcBlocked{c->src_blk}, col.source_colors, n,
+        pack_source_intensity_kernel<<<(unsigned)ceil_div(n, kThreads), kThreads, 0, st>>>(c->src_idx, col.source_colors, n,
                                                                                           c->sint);
         count_launch();
         ICP_CUDA(cudaGetLastError());
