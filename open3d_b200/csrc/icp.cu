@@ -1215,7 +1215,7 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     __shared__ double s_warp[kIcpThreads / 32][kSumStride];
     __shared__ double s_final[kSumStride];
     __shared__ float s_U[16];
-    __shared__ int s_done;
+    __shared__ int s_done, s_reverse;
     __shared__ __align__(8) unsigned long long s_mbar[kIcpThreads / 32][2];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     for (int k = threadIdx.x; k < (kIcpThreads / 32) * kSumStride; k += kIcpThreads) (&s_warp[0][0])[k] = 0.0;
@@ -1225,30 +1225,43 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     // block is still in its serial epilogue; nothing produced by that kernel is read before the wait.
     pdl_wait();
     pdl_launch_dependents();
-    if (threadIdx.x == 0) s_done = *(volatile int*)&a.st->done;
+    if (threadIdx.x == 0) {
+        s_done = *(volatile int*)&a.st->done;
+        s_reverse = a.st->executed & 1;
+    }
     if (threadIdx.x < 16) s_U[threadIdx.x] = a.st->Uf[threadIdx.x];
     __syncthreads();
     if (MODE == 0 && s_done) return;
 
-    // chunk c of this warp covers working-source positions [q0(c), q0(c) + 32); the arrays are padded to
-    // a multiple of 256 entries, so a chunk that starts below n can always be copied whole
+    // The warp owns the chunks starting at first, first + stride, ... below n (the arrays are padded to a multiple
+    // of 256 entries, so a chunk that starts below n can always be copied whole).  It visits them in ascending
+    // order when an even number of iterations has run and in descending order otherwise, so the evaluation pass
+    // sweeps opposite to the iteration before it.  An iteration touches about twice the L2 in records, seed rows
+    // and stores; walking the same order every time puts the whole working set between two uses of a line, while
+    // a reversed walk starts on what the previous launch touched last.  The order depends only on device state,
+    // never on how the host batches launches, and the per-chunk work is the same either way: only the order of the
+    // warp's f64 running sums changes.
     const int n = (int)a.n;
     const int stride = gridDim.x * kIcpThreads;
     const int first = blockIdx.x * kIcpThreads + w * 32;
+    const int steps = first < n ? (n - 1 - first) / stride + 1 : 0;
+    const int step = s_reverse ? -stride : stride;
+    const int start = s_reverse ? first + (steps - 1) * stride : first;
     constexpr unsigned kBytesA = kSrcChunkBytes;
     static_assert(offsetof(IcpStage<COLORED>, py) == 128 && offsetof(IcpStage<COLORED>, pz) == 256 &&
                   offsetof(IcpStage<COLORED>, jp) == 384 && offsetof(IcpStage<COLORED>, d2) == 512 &&
                   offsetof(IcpStage<COLORED>, ts) == kBytesA, "stage A mirrors a chunk record");
-    auto issue_a = [&](int c, int q0) {        // lane 0: ONE TMA bulk copy of chunk c's record into slot c & 1
-        if (lane == 0 && q0 < n) {
+    // chunk c (the warp's c-th step) covers working-source positions [start + c * step, ... + 32)
+    auto issue_a = [&](int c) {                // lane 0: ONE TMA bulk copy of chunk c's record into slot c & 1
+        if (lane == 0 && c < steps) {
             IcpStage<COLORED>& sl = sm.stage[w][c & 1];
             unsigned long long* mb = &s_mbar[w][c & 1];
             mbar_arrive_expect_tx(mb, kBytesA);
-            bulk_g2s(sl.px, a.src.chunk(q0), kBytesA, mb);
+            bulk_g2s(sl.px, a.src.chunk(start + c * step), kBytesA, mb);
         }
     };
-    auto issue_b = [&](int c, int q0) {        // every lane: gather its seed's rows of chunk c (needs A(c))
-        if (q0 < n) {
+    auto issue_b = [&](int c) {                // every lane: gather its seed's rows of chunk c (needs A(c))
+        if (c < steps) {
             IcpStage<COLORED>& sl = sm.stage[w][c & 1];
             mbar_wait(&s_mbar[w][c & 1], (unsigned)(c >> 1) & 1u);
             const int jp = sl.jp[lane];
@@ -1262,11 +1275,11 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     };
 
     double acc64 = 0.0;      // lane l: running total of slot l over this warp's queries
-    issue_a(0, first);
-    issue_a(1, first + stride);
-    issue_b(0, first);
-    int c = 0;
-    for (int q0 = first; q0 < n; q0 += stride, ++c) {
+    issue_a(0);
+    issue_a(1);
+    issue_b(0);
+    for (int c = 0; c < steps; ++c) {
+        const int q0 = start + c * step;
         IcpStage<COLORED>& sl = sm.stage[w][c & 1];
         // A(c) has landed: every lane waited on its mbarrier in issue_b(c), one trip ago (or in the prologue)
         cp_async_wait_all();                                       // B(c)
@@ -1274,8 +1287,8 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
         const int jp = sl.jp[lane];
         const float clear_prev = sl.d2[lane];
         __syncwarp();          // every lane has read its point / jp / d2 of slot c & 1: hand that part back to the producer
-        issue_a(c + 2, q0 + 2 * stride);
-        issue_b(c + 1, q0 + stride);
+        issue_a(c + 2);
+        issue_b(c + 1);
         // (ts / ns / cg of slot c & 1 are rewritten by issue_b(c + 2), i.e. in the NEXT trip: still valid below)
         const int i = q0 + lane;
         float term[32];
