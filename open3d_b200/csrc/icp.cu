@@ -834,6 +834,7 @@ struct IcpState {        // lives in device memory; read back once at the end
     int converged;
     int status;          // 0 ok, 1 singular
     unsigned ticket;
+    int sums_cached;     // chunk_sums holds every chunk's line for the working source as it is now (see IcpArgs)
 };
 
 struct IcpArgs {
@@ -845,6 +846,7 @@ struct IcpArgs {
                           // winner (-1 = none), clearance of that winner (lower bound on the distance to every OTHER
                           // target point, minus the motion since it was established; 0 = unknown)
     const int* src_idx;   // sorted source position -> original index (read in evaluate mode with corr_out only)
+    float* chunk_sums;    // per 32-query chunk, the 32 f32 sums its last iteration added to the warp's totals (128 B)
     int64_t n;            // local source points
     double n_total;       // source points over all ranks (fitness denominator)
     float rr, thr;
@@ -1066,9 +1068,16 @@ __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float*
 }
 
 // One chunk's contribution to the 30 sums: transposed warp reduction of the lanes' terms (f32 tree over 32
-// queries), added to the warp's running totals — one f64 per lane, lane l = slot l.
-__device__ __forceinline__ void icp_accumulate_chunk(float (&term)[32], bool matched, double& acc64) {
-    if (__any_sync(0xffffffffu, matched)) acc64 += (double)warp_transpose_sum32(term);
+// queries), added to the warp's running totals — one f64 per lane, lane l = slot l.  Returns what lane l added:
+// +0.0 when no lane matched, and adding +0.0 to acc64, which starts at +0.0 and so is never -0.0, leaves its bits
+// as they are.  A replayed chunk may therefore add its cached line unconditionally.
+__device__ __forceinline__ float icp_accumulate_chunk(float (&term)[32], bool matched, double& acc64) {
+    float line = 0.f;
+    if (__any_sync(0xffffffffu, matched)) {
+        line = warp_transpose_sum32(term);
+        acc64 += (double)line;
+    }
+    return line;
 }
 
 // The exchange step of the source-sharded loop (SURVEY.md 8e), done INSIDE the iteration kernel over NVLink /
@@ -1147,6 +1156,9 @@ __device__ __forceinline__ bool peer_all_reduce(const PeerView& pv, double* s_fi
 template <int MODE>
 __device__ __forceinline__ void icp_block_epilogue(const IcpArgs& a, double (*s_warp)[kSumStride], double* s_final) {
     if (!block_reduce_to_global<kIcpThreads>(s_warp, a.partials, &a.st->ticket, s_final)) return;
+    // Every other block has read sums_cached by now.  An iteration has just written or replayed the line of every
+    // chunk against the coordinates it left; the evaluation pass moves the coordinates and writes no line.
+    if (threadIdx.x == 0) a.st->sums_cached = MODE == 0;
     if (a.fuse_finalize) {
         if (threadIdx.x < 32) {
             if (a.use_peer && !peer_all_reduce(a.peer, s_final)) {
@@ -1199,6 +1211,10 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned by
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
+// through L2 only: for data an earlier launch wrote, which no L1 may hold a stale copy of
+__device__ __forceinline__ void cp_async16_cg(void* dst, const void* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
@@ -1215,7 +1231,7 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     __shared__ double s_warp[kIcpThreads / 32][kSumStride];
     __shared__ double s_final[kSumStride];
     __shared__ float s_U[16];
-    __shared__ int s_done, s_reverse;
+    __shared__ int s_done, s_reverse, s_cached;
     __shared__ __align__(8) unsigned long long s_mbar[kIcpThreads / 32][2];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     for (int k = threadIdx.x; k < (kIcpThreads / 32) * kSumStride; k += kIcpThreads) (&s_warp[0][0])[k] = 0.0;
@@ -1228,6 +1244,7 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     if (threadIdx.x == 0) {
         s_done = *(volatile int*)&a.st->done;
         s_reverse = a.st->executed & 1;
+        s_cached = MODE == 0 && a.st->sums_cached;
     }
     if (threadIdx.x < 16) s_U[threadIdx.x] = a.st->Uf[threadIdx.x];
     __syncthreads();
@@ -1260,15 +1277,39 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
             bulk_g2s(sl.px, a.src.chunk(start + c * step), kBytesA, mb);
         }
     };
+    // Sum replay (iterations only).  When the pending update leaves all of a chunk's points bit-for-bit where they
+    // were, every input of the chunk's sums is what the previous iteration used: the points, hence their exact
+    // nearest neighbours (every search path returns the exhaustive-search winner), hence the winners' rows and the
+    // per-handle constants.  Its 32 sums are then the line the previous iteration stored in a.chunk_sums, bit for
+    // bit, and adding that line to acc64 at the same place in the sweep gives the same totals.  Such a chunk fetches
+    // its 128-byte line instead of the seed rows, and does no search, no Jacobian, no reduction and no store.  Its
+    // seeds already hold the winners; only a clearance that a search would have re-established stays as it was,
+    // which can send a later search down another (equally exact) path.
+    bool replay_b = false;   // the decision of the last issue_b, warp-uniform
     auto issue_b = [&](int c) {                // every lane: gather its seed's rows of chunk c (needs A(c))
         if (c < steps) {
             IcpStage<COLORED>& sl = sm.stage[w][c & 1];
             mbar_wait(&s_mbar[w][c & 1], (unsigned)(c >> 1) & 1u);
-            const int jp = sl.jp[lane];
-            if (jp >= 0) {
-                cp_async16(&sl.ts[lane], a.tgt + jp);
-                if (MODE == 0) cp_async16(&sl.ns[lane], a.nrm + jp);
-                if (MODE == 0 && COLORED) cp_async16(&sl.cg[lane], a.tcg + jp);
+            const int q0 = start + c * step;
+            bool unchanged = true;   // (positions past n count as unchanged: the update moves padding points)
+            if (MODE == 0 && s_cached && q0 + lane < n) {
+                float x = sl.px[lane], y = sl.py[lane], z = sl.pz[lane];
+                const float ox = x, oy = y, oz = z;
+                apply_transform(s_U, x, y, z);   // the expression icp_process_query applies
+                unchanged = __float_as_uint(x) == __float_as_uint(ox) && __float_as_uint(y) == __float_as_uint(oy) &&
+                            __float_as_uint(z) == __float_as_uint(oz);
+            }
+            replay_b = MODE == 0 && s_cached && __all_sync(0xffffffffu, unchanged);
+            if (replay_b) {
+                if (lane < 8)
+                    cp_async16_cg(&sl.ts[lane], reinterpret_cast<const float4*>(a.chunk_sums + q0) + lane);
+            } else {
+                const int jp = sl.jp[lane];
+                if (jp >= 0) {
+                    cp_async16(&sl.ts[lane], a.tgt + jp);
+                    if (MODE == 0) cp_async16(&sl.ns[lane], a.nrm + jp);
+                    if (MODE == 0 && COLORED) cp_async16(&sl.cg[lane], a.tcg + jp);
+                }
             }
         }
         cp_async_commit();
@@ -1281,8 +1322,9 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     for (int c = 0; c < steps; ++c) {
         const int q0 = start + c * step;
         IcpStage<COLORED>& sl = sm.stage[w][c & 1];
+        const bool replay = replay_b;
         // A(c) has landed: every lane waited on its mbarrier in issue_b(c), one trip ago (or in the prologue)
-        cp_async_wait_all();                                       // B(c)
+        cp_async_wait_all();                                       // B(c), or the cached line of chunk c
         const float px = sl.px[lane], py = sl.py[lane], pz = sl.pz[lane];
         const int jp = sl.jp[lane];
         const float clear_prev = sl.d2[lane];
@@ -1290,6 +1332,10 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
         issue_a(c + 2);
         issue_b(c + 1);
         // (ts / ns / cg of slot c & 1 are rewritten by issue_b(c + 2), i.e. in the NEXT trip: still valid below)
+        if (replay) {
+            acc64 += (double)reinterpret_cast<const float*>(sl.ts)[lane];
+            continue;
+        }
         const int i = q0 + lane;
         float term[32];
 #pragma unroll
@@ -1298,7 +1344,8 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
         if (i < n)
             matched = icp_process_query<L2LOSS, MODE, COLORED>(a, s_U, i, px, py, pz, jp, clear_prev, &sl.ts[lane],
                                                                &sl.ns[lane], &sl.cg[COLORED ? lane : 0], term);
-        icp_accumulate_chunk(term, matched, acc64);
+        const float line = icp_accumulate_chunk(term, matched, acc64);
+        if (MODE == 0) a.chunk_sums[q0 + lane] = line;   // one coalesced 128-byte store
     }
     if (lane < kNumSums) s_warp[w][lane] = acc64;
     icp_block_epilogue<MODE>(a, s_warp, s_final);
@@ -1332,6 +1379,7 @@ struct o3db_icp {
     double init_T[16];
     char* src_blk = nullptr;         // chunk-blocked working source: points, seeds, clearances (SrcBlocked)
     int* src_idx = nullptr;          // sorted source position -> original index
+    float* chunk_sums = nullptr;     // n_pad floats: one 128-byte line of cached sums per 32-query chunk (IcpArgs)
     unsigned* src_key = nullptr;     // cell key of every source point (sort order)
     unsigned* src_rank = nullptr;
     unsigned* src_start = nullptr;   // CSR offsets of the source sort
@@ -1380,6 +1428,7 @@ static IcpArgs make_args(o3db_icp* c) {
     a.cs = c->nns.cell_start;
     a.src = SrcBlocked{c->src_blk};
     a.src_idx = c->src_idx;
+    a.chunk_sums = c->chunk_sums;
     a.n = c->n;
     a.n_total = c->n_total;
     const float r = (float)c->opt.max_correspondence_distance;
@@ -1410,7 +1459,7 @@ static IcpArgs make_args(o3db_icp* c) {
 }
 
 static int icp_init_state(o3db_icp* c, cudaStream_t st) {
-    IcpState h{};
+    IcpState h{};   // (sums_cached = 0: o3db_icp_reset has just gathered the caller's source again, which may differ)
     for (int i = 0; i < 16; ++i) {
         h.T[i] = c->init_T[i];
         h.Uf[i] = (i % 5 == 0) ? 1.f : 0.f;   // the initial transform is applied by the gather
@@ -1724,6 +1773,7 @@ void o3db_icp_destroy(o3db_icp* c) {
     nns_free(&c->nns, st);
     if (c->src_blk) cudaFreeAsync(c->src_blk, st);
     if (c->src_idx) cudaFreeAsync(c->src_idx, st);
+    if (c->chunk_sums) cudaFreeAsync(c->chunk_sums, st);
     if (c->src_key) cudaFreeAsync(c->src_key, st);
     if (c->src_rank) cudaFreeAsync(c->src_rank, st);
     if (c->src_start) cudaFreeAsync(c->src_start, st);
@@ -1812,6 +1862,8 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     c->n_pad = ceil_div(n, 256) * 256;
     ICP_CUDA(cudaMallocAsync(&c->src_blk, SrcBlocked::bytes(c->n_pad), st));
     ICP_CUDA(cudaMallocAsync(&c->src_idx, c->n_pad * sizeof(int), st));
+    // (no initial contents: IcpState::sums_cached starts at 0, so the first iteration writes every line)
+    ICP_CUDA(cudaMallocAsync(&c->chunk_sums, c->n_pad * sizeof(float), st));
     src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlocked{c->src_blk}, n, c->n_pad, true);
     count_launch();
     ICP_CUDA(cudaGetLastError());
