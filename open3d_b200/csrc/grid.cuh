@@ -300,22 +300,31 @@ __device__ __forceinline__ float dist2_canonical(const float4 t, float qx, float
 // kernel fetched the seed one chunk ahead and needs the distance for its certificate).  The box [q - rad,
 // q + rad], rad = sqrt(sd) (hardware reciprocal square root, 2 ulp, with a 1e-4 margin), is scanned from
 // "nothing yet": it contains the seed, hence the exact winner and every point tying with it.
-// On return `handled` = false when the fast path does not apply (box taller than 3 cell rows, long slabs:
-// the caller then calls nn_search_slow); otherwise the winner's sorted position is returned and
-// `clearance` = a lower bound on the distance from the query to EVERY target point other than the winner:
-// min(sqrt(d2nd), rad) — a point that was not scanned lies outside the box, i.e. farther than rad along
-// grid-y or grid-z (binning is monotone; lo_bound / hi_bound only widen the box).
+// A seed farther than r1 (right after a large update: the old winner is a motion's length away while the true
+// neighbour is millimetres away) would bound a box larger than the unseeded search's pass 1, often taller than 3
+// cell rows; the box is then pass 1's, [q - r1, q + r1], and its best point is the exact winner when it lies within
+// r1 (r1_accept2 = (r1 (1 - 1e-4))^2, as in nn_search_slow): every point outside the box is farther than r1.
+// Fewer candidates is what saves time in these iterations, whose scans are bound by the instructions every candidate
+// costs (DESIGN.md §4.1); and the query leaves with a clearance, where nn_search_slow leaves none.
+// On return `handled` = false when the fast path does not apply (box taller than 3 cell rows, long slabs, or the
+// best point of pass 1's box not within r1: the caller then calls nn_search_slow); otherwise the winner's sorted
+// position is returned and `clearance` = a lower bound on the distance from the query to EVERY target point other
+// than the winner: min(sqrt(d2nd), rad) — a point that was not scanned lies outside the box, i.e. farther than rad
+// along grid-y or grid-z (binning is monotone; lo_bound / hi_bound only widen the box).
 __device__ __forceinline__ unsigned nn_search_seeded_fast(const Grid& g, const float4* __restrict__ pts,
                                                           const unsigned* __restrict__ cs, float qx, float qy,
-                                                          float qz, float rr, float thr, float sd, bool& handled,
-                                                          float& clearance) {
-    const float rad = sd > 0.f ? fminf(rr, sd * rsqrtf(sd) * 1.0001f) : 0.f;
+                                                          float qz, float r1, float r1_accept2, float rr, float thr,
+                                                          float sd, bool& handled, float& clearance) {
+    const float rs = sd > 0.f ? fminf(rr, sd * rsqrtf(sd) * 1.0001f) : 0.f;
+    const bool far = rs > r1;
+    const float rad = far ? r1 : rs;
     float gx, gy, gz;
     to_grid(g, qx, qy, qz, gx, gy, gz);
     unsigned long long best = ((unsigned long long)__float_as_uint(thr) << 32) | 0x7fffffffull;
     unsigned bj = kNoPoint;
     float d2nd = __int_as_float(0x7f7fffff);
-    handled = scan_box_flat<3, true>(g, pts, cs, gy, gz, qx, qy, qz, rad, best, bj, &d2nd);
+    handled = scan_box_flat<3, true>(g, pts, cs, gy, gz, qx, qy, qz, rad, best, bj, &d2nd) &&
+              (!far || (bj != kNoPoint && __uint_as_float((unsigned)(best >> 32)) <= r1_accept2));
     // rounded down: 2 ulp of the reciprocal square root and the f32 rounding of d2nd are inside the 1e-5
     clearance = fminf(rad, d2nd * rsqrtf(fmaxf(d2nd, 1e-37f)) * 0.99999f);
     return bj;

@@ -1031,7 +1031,8 @@ __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float*
                 clear_new = clear;
                 handled = true;
             } else {
-                bj = nn_search_seeded_fast(a.g, a.tgt, a.cs, px, py, pz, a.rr, a.thr, sd, handled, clear_new);
+                bj = nn_search_seeded_fast(a.g, a.tgt, a.cs, px, py, pz, a.r1, a.r1_accept2, a.rr, a.thr, sd, handled,
+                                           clear_new);
             }
         }
     }
