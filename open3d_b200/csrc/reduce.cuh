@@ -1,7 +1,9 @@
 // reduce.cuh — the 29(+1)-scalar Gauss-Newton reduction shared by the ICP kernels (icp.cu) and RGB-D
 // odometry (odometry.cu): per-thread f32 partials -> f64 warp tree -> per-warp shared-memory slots ->
-// per-block partials -> last block (atomic ticket) sums in block order; plus the f64 6x6 solve and
-// pose -> transformation that the reference runs on the host (kernel/TransformationConverter.cpp).
+// per-block partials -> last block (atomic ticket) sums in block order, with reduce_sums the whole loop of the
+// stand-alone reductions; plus the f64 6x6 solve and pose -> transformation that the reference runs on the host
+// (kernel/TransformationConverter.cpp), and the on-device Gauss-Newton step built from them
+// (gauss_newton_step_warp, left_multiply_warp) that the fused ICP and odometry loops run on one warp.
 #pragma once
 
 #include <utility>
@@ -105,6 +107,31 @@ __device__ __forceinline__ bool block_reduce_to_global(double (*s_warp)[kSumStri
     if (threadIdx.x == 0) *ticket = 0;
     __syncthreads();
     return true;
+}
+
+// The whole reduction of a kThreads-thread block over elements [0, n): a grid-stride loop in which each thread calls
+// body(i, acc) for its element i < n of every kThreads-wide stride, body adding that element's terms to the f32
+// partials acc; flush_acc into s_warp (zeroed here) every kFlushEvery strides and once at the end; then
+// block_reduce_to_global.  All threads of the block must call it.  Returns true in the last block, with s_final[] filled.
+template <typename Body>
+__device__ __forceinline__ bool reduce_sums(int64_t n, double (*s_warp)[kSumStride], double* __restrict__ partials,
+                                            unsigned* ticket, double* s_final, Body&& body) {
+    for (int k = threadIdx.x; k < (kThreads / 32) * kSumStride; k += kThreads) (&s_warp[0][0])[k] = 0.0;
+    __syncthreads();
+    float acc[kNumSums];
+#pragma unroll
+    for (int k = 0; k < kNumSums; ++k) acc[k] = 0.f;
+    int since = 0;
+    for (int64_t base = (int64_t)blockIdx.x * kThreads; base < n; base += (int64_t)gridDim.x * kThreads) {
+        const int64_t i = base + threadIdx.x;
+        if (i < n) body(i, acc);
+        if (++since == kFlushEvery) {
+            flush_acc(acc, s_warp);
+            since = 0;
+        }
+    }
+    flush_acc(acc, s_warp);
+    return block_reduce_to_global(s_warp, partials, ticket, s_final);
 }
 
 // --------------------------------------------------------- 6x6 solve (f64)
@@ -217,24 +244,54 @@ __device__ __forceinline__ bool solve6x6_warp(const double* __restrict__ A, doub
 // same expressions as the single-thread path.
 __device__ __host__ inline void pose_to_T_trig(const double* p, double ca, double sa, double cb, double sb, double cg,
                                                double sg, double* T) {
-    for (int i = 0; i < 16; ++i) T[i] = 0.0;
-    T[15] = 1.0;
     T[0] = cg * cb;
     T[1] = -1 * sg * ca + cg * sb * sa;
     T[2] = sg * sa + cg * sb * ca;
+    T[3] = p[3];
     T[4] = sg * cb;
     T[5] = cg * ca + sg * sb * sa;
     T[6] = -1 * cg * sa + sg * sb * ca;
+    T[7] = p[4];
     T[8] = -1 * sb;
     T[9] = cb * sa;
     T[10] = cb * ca;
-    T[3] = p[3];
-    T[7] = p[4];
     T[11] = p[5];
+    T[12] = T[13] = T[14] = 0.0;
+    T[15] = 1.0;
 }
 
 __device__ __host__ inline void pose_to_T(const double* p, double* T) {
     pose_to_T_trig(p, cos(p[0]), sin(p[0]), cos(p[1]), sin(p[1]), cos(p[2]), sin(p[2]), T);
+}
+
+// -------------------------------------------------- Gauss-Newton step on one warp
+
+// The on-device part of one Gauss-Newton step, by ONE warp (all 32 lanes must call it): the 29 f64 sums ->
+// solve6x6_warp -> the six cos / sin of the pose on six lanes -> the update U = pose_to_T_trig on lane 0.
+// `scratch` is 64 doubles of shared memory: the pose in [0, 6), cos a, cos b, cos g, sin a, sin b, sin g in [8, 14),
+// the solve's matrix in [16, 58), and U in [16, 32) (the matrix is dead by then), where the caller reads it.
+// Returns false on every lane for a singular system, and then leaves U unwritten.
+__device__ __forceinline__ bool gauss_newton_step_warp(const double* sums, double* scratch) {
+    const int lane = threadIdx.x & 31;
+    double* pose = scratch;
+    double* trig = scratch + 8;
+    if (!solve6x6_warp(sums, scratch + 16, pose)) return false;
+    if (lane < 3) trig[lane] = cos(pose[lane]);
+    else if (lane < 6) trig[lane] = sin(pose[lane - 3]);
+    __syncwarp();
+    if (lane == 0) pose_to_T_trig(pose, trig[0], trig[3], trig[1], trig[4], trig[2], trig[5], scratch + 16);
+    __syncwarp();
+    return true;
+}
+
+// T <- U T for 4 x 4 row-major matrices, by lanes 0-15 of a warp (all sixteen must call it): lane l writes T[l].
+__device__ __forceinline__ void left_multiply_warp(const double* U, double* T) {
+    const int lane = threadIdx.x & 31, i = lane >> 2, j = lane & 3;
+    double v = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) v += U[i * 4 + k] * T[k * 4 + j];
+    __syncwarp(0xffffu);   // every lane has read the old T
+    T[lane] = v;
 }
 
 }  // namespace o3db
