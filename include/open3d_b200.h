@@ -462,6 +462,25 @@ int o3db_vbg_ray_cast(o3db_vbg* vbg, const int32_t* block_coords_dev, int64_t nu
                       int range_map_down_factor, float* range_dev, void* stream);
 
 /* ------------------------------------------------------------------------
+ * VoxelBlockGrid::ExtractPointCloud (t/geometry/VoxelBlockGrid.cpp:404-434; slam::Model::ExtractPointCloud,
+ * slam/Model.cpp:108-111, forwards to it) = BufferRadiusNeighbors (VoxelBlockGrid.cpp:22-51) + kernel::voxel_grid::
+ * ExtractPointCloud (kernel/VoxelBlockGridImpl.h:1122-1381): one point per voxel o and axis i where o and o + e_i both
+ * have weight > weight_threshold and tsdf_i * tsdf_o < 0, at the linear zero crossing, with the interpolated TSDF
+ * gradient as normal and the interpolated colour / 255 (grids with colour only).
+ *
+ * Rows come in a deterministic order (upstream's is an atomic counter's): ascending block slot (the order of
+ * o3db_vbg_active_indices), then the linear voxel index (z*R + y)*R + x, then axis 0, 1, 2; two calls on an unchanged
+ * volume give identical bits.  max_points < 0: every point (upstream's estimated_point_number = -1); max_points >= 0:
+ * the first min(max_points, total) rows of that order.  The surface may hold at most INT32_MAX points.
+ *
+ * Outputs: *num_points and [*num_points, 3] f32 device buffers owned by the handle, valid until the next extract on
+ * it or o3db_vbg_destroy; *colors is NULL for a grid without colour, all three are NULL when there are no points.
+ * Synchronises the stream once (the point count); reports a frame dropped for capacity like o3db_vbg_size.
+ * ---------------------------------------------------------------------- */
+int o3db_vbg_extract_point_cloud(o3db_vbg* vbg, float weight_threshold, int64_t max_points, int64_t* num_points,
+                                 float** points, float** normals, float** colors, void* stream);
+
+/* ------------------------------------------------------------------------
  * RGB-D odometry, PointToPlane method — slam::Model::TrackFrameToModel (slam/Model.cpp:68-89) ->
  * odometry::RGBDOdometryMultiScale (odometry/RGBDOdometry.cpp:56-206).
  *

@@ -140,6 +140,8 @@ _SIGS = {
     "o3db_vbg_estimate_range": (_i, [_vp, _vp, _i64, _dp, _dp, _i, _i, _i, _f, _f, _vp, _vp]),
     "o3db_vbg_ray_cast": (_i, [_vp, _vp, _i64, _dp, _dp, _i, _i, C.POINTER(RaycastOutputs), _f, _f, _f, _f, _f, _i,
                                _vp, _vp]),
+    "o3db_vbg_extract_point_cloud": (_i, [_vp, _f, _i64, C.POINTER(_i64), C.POINTER(_vp), C.POINTER(_vp),
+                                          C.POINTER(_vp), _vp]),
     "o3db_vbg_profile": (_i, [_vp, _i]),
     "o3db_vbg_profile_read": (_i, [_vp, _dp, _dp, C.POINTER(_i64)]),
     "o3db_build_spatial_hash_table": (_i, [_vp, _i64, _dbl, C.c_uint32, _vp, _vp, _vp]),

@@ -15,6 +15,7 @@
 #include "common.cuh"
 #include "grid.cuh"
 #include "reduce.cuh"
+#include "scan.cuh"
 
 namespace o3db {
 
@@ -203,9 +204,7 @@ __global__ void scatter_kernel(const float* __restrict__ pts, const float* __res
     if (nrm4) nrm4[p] = make_float4(nrm[3 * i], nrm[3 * i + 1], nrm[3 * i + 2], 0.f);
 }
 
-// Exclusive scan of u32 data[0..n) in place; data[n] receives the total.
-static constexpr int kScanItems = 8;
-static constexpr int kScanTile = kThreads * kScanItems;
+// Exclusive scan of u32 data[0..n) in place; data[n] receives the total (scan.cuh).
 
 __device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned& total) {
     __shared__ unsigned s_w[kThreads / 32];
@@ -277,7 +276,7 @@ __global__ void scan_apply(unsigned* __restrict__ data, int64_t n, const unsigne
 }
 
 // data has n+1 entries; scratch has ceil(n/kScanTile) entries.
-static int exclusive_scan_u32(unsigned* data, int64_t n, unsigned* scratch, cudaStream_t st) {
+int exclusive_scan_u32(unsigned* data, int64_t n, unsigned* scratch, cudaStream_t st) {
     const int64_t ntiles = ceil_div(n, kScanTile);
     scan_tile_sums<<<(unsigned)ntiles, kThreads, 0, st>>>(data, n, scratch);
     O3DB_LAUNCH_CHECK();

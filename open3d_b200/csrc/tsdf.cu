@@ -992,7 +992,7 @@ static int grow(o3db_vbg* v, int64_t new_capacity, cudaStream_t st) {
     return O3DB_OK;
 }
 
-static int absorb_status(o3db_vbg* v, const int* h) {
+int absorb_status(o3db_vbg* v, const int* h) {
     v->known_size = h[0];
     v->max_new_seen = std::max<int64_t>(v->max_new_seen, h[9]);
     if (h[6]) {
@@ -1200,6 +1200,7 @@ void o3db_vbg_destroy(o3db_vbg* v) {
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (v->h_pinned) pinned_release(v->h_pinned);
+    extract_release(v);
     for (auto& e : v->ev)
         if (e) cudaEventDestroy(e);
     for (auto& e : v->prof_ev)

@@ -126,4 +126,23 @@ struct o3db_vbg {
     std::vector<cudaEvent_t> prof_ev;
     int64_t prof_frames = 0;
     bool prof_on = false;
+    // o3db_vbg_extract_point_cloud (extract.cu): scratch for ext_blocks slots, outputs for ext_rows points
+    int64_t ext_blocks = 0;
+    int* ext_nb = nullptr;                    // [ext_blocks][27] neighbour slots, -1 = absent
+    unsigned* ext_counts = nullptr;           // [ext_blocks + 1] points per block, then their exclusive scan
+    unsigned* ext_scan = nullptr;             // scan tile sums
+    unsigned* ext_masks = nullptr;            // [ext_blocks][ceil(res^3 / 32)][3] crossing bits per axis
+    unsigned long long* ext_total = nullptr;  // 64-bit point count
+    long long* h_ext_total = nullptr;         // pinned read-back of it
+    int64_t ext_rows = 0;
+    float* ext_points = nullptr;
+    float* ext_normals = nullptr;
+    float* ext_colors = nullptr;
 };
+
+namespace o3db {
+// tsdf.cu: takes the status words size_dev[0..15] read back into h; O3DB_ERR_CAPACITY after a dropped frame
+int absorb_status(o3db_vbg* v, const int* h);
+// extract.cu: frees what o3db_vbg_extract_point_cloud allocated (o3db_vbg_destroy, after a device synchronise)
+void extract_release(o3db_vbg* v);
+}  // namespace o3db

@@ -459,6 +459,25 @@ class VoxelBlockGrid:
         out["range"] = rng
         return out
 
+    def extract_point_cloud(self, weight_threshold=3.0, estimated_point_number=-1):
+        """VoxelBlockGrid::ExtractPointCloud (VoxelBlockGrid.cpp:404-434; pybind voxel_block_grid.cpp:180-183): the
+        zero crossings of the TSDF between voxels of weight > weight_threshold, as a PointCloud with "positions",
+        "normals" and, when the grid has colour, "colors".  Rows in a fixed order (block slot, voxel, axis; see
+        o3db_vbg_extract_point_cloud); estimated_point_number >= 0 keeps the first that many."""
+        n = C.c_int64(0)
+        pts, nrm, col = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        self._replay.guard(lambda: check(lib.o3db_vbg_extract_point_cloud(
+            self._h, float(weight_threshold), int(estimated_point_number), C.byref(n), C.byref(pts), C.byref(nrm),
+            C.byref(col), current_stream_ptr())))
+        rows = int(n.value)
+        # the library's buffers are reused by the next call: copy out
+        out = PointCloud()
+        out.point["positions"] = _s.device_view(pts.value, (rows, 3), torch.float32).clone()
+        out.point["normals"] = _s.device_view(nrm.value, (rows, 3), torch.float32).clone()
+        if self._with_color:
+            out.point["colors"] = _s.device_view(col.value, (rows, 3), torch.float32).clone()
+        return out
+
     def last_frustum_block_coordinates(self):
         cap = 76800
         out = torch.empty((cap, 3), dtype=torch.int32, device="cuda")
