@@ -186,6 +186,30 @@ int o3db_estimate_color_gradients_solver(const float* positions_dev, const float
                                          const float* colors_dev, int64_t n, double radius, int max_nn,
                                          int solver, float* color_gradients_dev /* [n,3] */, void* stream);
 
+/* t::geometry::PointCloud::EstimateNormals(max_nn, radius) with the hybrid search (t/geometry/PointCloud.cpp:856-984,
+ * kernel/PointCloudImpl.h:512-638 and 746-1065): the hybrid search of the cloud on itself, then per point the
+ * covariance of its neighbours (f64 sums, Bessel's correction, stored f32; identity below 3 neighbours) and the
+ * normal of the reference's fast 3x3 eigen solve, oriented as upstream:
+ *   has_normals == 0: normals_dev is output only; a zero normal becomes (0,0,1);
+ *   has_normals != 0: normals_dev holds the prior normals on entry; the new normal is flipped where its dot with
+ *     the prior is negative, and a zero normal stays zero.
+ * covariances_dev ([n,9] row-major, may be NULL) receives upstream's transient "covariances" attribute.  The
+ * covariances are bit-identical to the reference's CPU kernel on identical neighbour lists; the normals differ only
+ * where libm's acosf / cosf are not correctly rounded (DESIGN.md).  max_nn in 1..32 (reference default 30); n == 0 is
+ * a no-op.  Synchronises the stream. */
+int o3db_estimate_normals(const float* positions_dev, int64_t n, double radius, int max_nn, int has_normals,
+                          float* normals_dev /* [n,3] */, float* covariances_dev /* [n,9] or NULL */, void* stream);
+
+/* PointCloud::OrientNormalsToAlignWithDirection (PointCloudImpl.h:261-294): in place, a normal whose dot with
+ * direction is negative is flipped and a zero normal becomes direction. */
+int o3db_orient_normals_to_align_with_direction(float* normals_dev, int64_t n, const float direction_host[3],
+                                                void* stream);
+
+/* PointCloud::OrientNormalsTowardsCameraLocation (PointCloudImpl.h:296-351): in place, a normal that points away from
+ * camera - p is flipped; a zero normal becomes (camera - p) / |camera - p|, or (0,0,1) where that is zero. */
+int o3db_orient_normals_towards_camera_location(const float* positions_dev, float* normals_dev, int64_t n,
+                                                const float camera_host[3], void* stream);
+
 /* ------------------------------------------------------------------------
  * Fused, device-resident ICP loop — replaces
  * t::pipelines::registration::ICP / MultiScaleICP / DoSingleScaleICPIterations /

@@ -82,6 +82,9 @@ _SIGS = {
                                           _vp]),
     "o3db_estimate_color_gradients": (_i, [_vp, _vp, _vp, _i64, _dbl, _i, _vp, _vp]),
     "o3db_estimate_color_gradients_solver": (_i, [_vp, _vp, _vp, _i64, _dbl, _i, _i, _vp, _vp]),
+    "o3db_estimate_normals": (_i, [_vp, _i64, _dbl, _i, _i, _vp, _vp, _vp]),
+    "o3db_orient_normals_to_align_with_direction": (_i, [_vp, _i64, _vp, _vp]),
+    "o3db_orient_normals_towards_camera_location": (_i, [_vp, _vp, _i64, _vp, _vp]),
     "o3db_icp_create_colored": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions), _dbl, _vp,
                                      _vp, C.POINTER(_vp)]),
     "o3db_icp_colored": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions), _dbl,

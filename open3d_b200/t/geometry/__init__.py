@@ -107,6 +107,63 @@ class PointCloud:
         self.point["color_gradients"] = g
         return self
 
+    def estimate_normals(self, max_nn=30, radius=None):
+        """PointCloud::EstimateNormals (t/geometry/PointCloud.cpp:856-984), hybrid search: sets "normals" in place.
+        If the cloud already has normals, each new normal is flipped where it points against the old one, as
+        upstream does; otherwise a point whose normal cannot be estimated gets (0, 0, 1)."""
+        p = self._positions_f32("EstimateNormals")
+        if radius is None or max_nn is None:
+            raise RuntimeError("open3d_b200 builds the hybrid-search variant: pass max_nn and radius (upstream's "
+                               "KNN-only and radius-only variants are outside this build's scope).")
+        n = int(p.shape[0])
+        has_normals = self.has_point_normals()
+        if has_normals:
+            nrm = self._normals_f32(n)
+        else:
+            nrm = torch.empty_like(p)
+        check(lib.o3db_estimate_normals(p.data_ptr(), n, float(radius), int(max_nn), int(has_normals), nrm.data_ptr(),
+                                        None, current_stream_ptr()))
+        self.point["normals"] = nrm
+        return self
+
+    def orient_normals_to_align_with_direction(self, orientation_reference=(0.0, 0.0, 1.0)):
+        """PointCloud::OrientNormalsToAlignWithDirection (t/geometry/PointCloud.cpp:986-1018): in place."""
+        d = _vec3_f32(orientation_reference, "orientation_reference")
+        if not self.has_point_normals():
+            raise RuntimeError("No normals in the PointCloud. Call EstimateNormals() first.")
+        nrm = self._normals_f32(int(self._positions_f32("OrientNormalsToAlignWithDirection").shape[0]))
+        check(lib.o3db_orient_normals_to_align_with_direction(nrm.data_ptr(), int(nrm.shape[0]), d.ctypes.data,
+                                                              current_stream_ptr()))
+        self.point["normals"] = nrm
+        return self
+
+    def orient_normals_towards_camera_location(self, camera_location=(0.0, 0.0, 0.0)):
+        """PointCloud::OrientNormalsTowardsCameraLocation (t/geometry/PointCloud.cpp:1020-1051): in place."""
+        c = _vec3_f32(camera_location, "camera_location")
+        if not self.has_point_normals():
+            raise RuntimeError("No normals in the PointCloud. Call EstimateNormals() first.")
+        p = self._positions_f32("OrientNormalsTowardsCameraLocation")
+        nrm = self._normals_f32(int(p.shape[0]))
+        check(lib.o3db_orient_normals_towards_camera_location(p.data_ptr(), nrm.data_ptr(), int(nrm.shape[0]),
+                                                              c.ctypes.data, current_stream_ptr()))
+        self.point["normals"] = nrm
+        return self
+
+    def _positions_f32(self, who):
+        p = self.point.get("positions")
+        if p is None:
+            raise RuntimeError(f"{who}: the PointCloud has no positions.")
+        if p.dtype != torch.float32:
+            # upstream also takes Float64; this build implements Float32
+            raise RuntimeError(f"{who}: only Float32 point clouds are supported by open3d_b200 (got {p.dtype})")
+        return p.contiguous()
+
+    def _normals_f32(self, n):
+        nrm = self.point["normals"]
+        if nrm.dtype != torch.float32 or nrm.dim() != 2 or nrm.shape[1] != 3 or nrm.shape[0] != n:
+            raise RuntimeError(f"normals must be [{n}, 3] Float32, as the positions (got {tuple(nrm.shape)} {nrm.dtype})")
+        return nrm.contiguous()
+
     def transform(self, transformation):
         """PointCloud::Transform (t/geometry/PointCloud.cpp:352-371): in place on
         positions and, if present, normals."""
@@ -248,6 +305,16 @@ def _color_dtype(t):
     if t.dtype == torch.float32:
         return COLOR_F32
     raise RuntimeError(f"Unsupported color image dtype {t.dtype}")
+
+
+def _vec3_f32(v, name):
+    # the reference takes a 3-vector tensor and casts it to the cloud's dtype (PointCloud.cpp:990-996)
+    if isinstance(v, torch.Tensor):
+        v = v.detach().cpu().numpy()
+    v = np.ascontiguousarray(np.asarray(v).astype(np.float32))
+    if v.shape != (3,):
+        raise RuntimeError(f"{name}: expected shape {{3}}, got {v.shape}")
+    return v
 
 
 def _k9(K):
