@@ -505,6 +505,42 @@ int o3db_vbg_extract_point_cloud(o3db_vbg* vbg, float weight_threshold, int64_t 
                                  float** points, float** normals, float** colors, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Point clouds from depth / RGB-D images and back (t/geometry/kernel/ paths).
+ *
+ * o3db_unproject: PointCloud::CreateFromDepthImage / CreateFromRGBDImage without normals (t/geometry/PointCloud.cpp:
+ * 1414-1469) -> kernel::pointcloud::Unproject (kernel/PointCloud.cpp:21-65, kernel/PointCloudImpl.h:43-144).  The
+ * strided grid is (rows / stride) x (cols / stride); strided pixel (i, j) is image pixel (x, y) = (j*stride, i*stride)
+ * with d = depth / depth_scale; it gives a point when 0 < d < depth_max, at RigidTransform(InverseTransformation(
+ * extrinsic), Unproject(x, y, d)) in f32, and, with a colour image, the colour pixel at (x, y) as f32 without scaling
+ * (a u8 image gives 0..255, as upstream's rgbd.color_.To(Float32)).  Rows come row-major over the strided grid
+ * (upstream's order is an atomic counter's); two calls give identical bits.  points_dev / colors_dev need room for
+ * the whole strided grid; *num_points receives the count (one stream synchronise).
+ *
+ * o3db_project: PointCloud::ProjectToDepthImage / ProjectToRGBDImage (PointCloud.cpp:1471-1530) ->
+ * kernel::pointcloud::Project (kernel/PointCloudCUDA.cu:26-162).  A point is moved by extrinsic, projected, and
+ * u, v rounded half away from zero; it is rejected when !InBoundary(u, v) || zc <= 0 || zc > depth_max.  Each pixel
+ * takes the point with the least (float bits of d = zc * depth_scale, point index), the reference CUDA kernel's
+ * packed atomicMin, for depth-only images too; every pixel of depth_dev ([rows][cols] f32) and color_dev
+ * ([rows][cols][3] f32, with colors_dev) is written, 0 where no point lands.  The reference CPU kernel
+ * (PointCloudCPU.cpp:21-90) differs at an exact depth tie, where it keeps the colour of the last writer.
+ * Asynchronous.
+ *
+ * Unlike upstream, both reject (O3DB_ERR_INVALID) null pointers, stride < 1, a depth_scale that is not finite and
+ * positive, negative image sizes, a strided grid or point count of 2^31 or more, and colour dtypes other than
+ * O3DB_COLOR_U8 / O3DB_COLOR_F32.  Each call runs a fixed number of kernels, whatever its sizes.
+ * ---------------------------------------------------------------------- */
+int o3db_unproject(const void* depth_dev, int depth_dtype, int rows, int cols,
+                   const void* color_dev /* NULL or [rows][cols][3] */, int color_dtype,
+                   const double intrinsic_host[9], const double extrinsic_host[16],
+                   float depth_scale, float depth_max, int stride,
+                   float* points_dev, float* colors_dev /* [(rows/stride)*(cols/stride)][3] */,
+                   int64_t* num_points, void* stream);
+int o3db_project(const float* points_dev, const float* colors_dev /* NULL: depth only */, int64_t n,
+                 const double intrinsic_host[9], const double extrinsic_host[16],
+                 float depth_scale, float depth_max, int rows, int cols,
+                 float* depth_dev /* [rows][cols] */, float* color_dev /* [rows][cols][3] or NULL */, void* stream);
+
+/* ------------------------------------------------------------------------
  * RGB-D odometry, PointToPlane method — slam::Model::TrackFrameToModel (slam/Model.cpp:68-89) ->
  * odometry::RGBDOdometryMultiScale (odometry/RGBDOdometry.cpp:56-206).
  *

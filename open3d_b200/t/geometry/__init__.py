@@ -149,6 +149,102 @@ class PointCloud:
         self.point["normals"] = nrm
         return self
 
+    @staticmethod
+    def create_from_depth_image(depth, intrinsics, extrinsics=None, depth_scale=1000.0, depth_max=3.0, stride=1,
+                                with_normals=False):
+        """PointCloud::CreateFromDepthImage (t/geometry/PointCloud.cpp:1414-1442; pybind pointcloud.cpp:451-473): one
+        point per strided pixel with 0 < depth / depth_scale < depth_max, in the world frame of extrinsics (default
+        identity).  depth: Image, torch tensor or numpy array, [H,W] or [H,W,1] UInt16 / Float32.  Rows row-major over
+        the strided grid (see o3db_unproject)."""
+        return PointCloud._unproject(depth, None, intrinsics, extrinsics, depth_scale, depth_max, stride, with_normals)
+
+    @staticmethod
+    def create_from_rgbd_image(rgbd_image, intrinsics, extrinsics=None, depth_scale=1000.0, depth_max=3.0, stride=1,
+                               with_normals=False):
+        """PointCloud::CreateFromRGBDImage (PointCloud.cpp:1444-1469; pybind pointcloud.cpp:474-497): as
+        create_from_depth_image, plus "colors" = the [H,W,3] UInt8 / Float32 colour pixel as Float32 without scaling
+        (0..255 for UInt8, as upstream's color.To(Float32))."""
+        return PointCloud._unproject(rgbd_image.depth, rgbd_image.color, intrinsics, extrinsics, depth_scale,
+                                     depth_max, stride, with_normals)
+
+    @staticmethod
+    def _unproject(depth, color, intrinsics, extrinsics, depth_scale, depth_max, stride, with_normals):
+        if with_normals:
+            raise RuntimeError("with_normals=True is not built in open3d_b200: upstream's path filters the depth with "
+                               "NPP's bilateral filter or PyrDown first, which this build does not reproduce. Create "
+                               "the cloud without normals and call estimate_normals().")
+        K = _k9(intrinsics)
+        E = as_host_f64_4x4(np.eye(4) if extrinsics is None else extrinsics, "extrinsics")
+        d = _image_tensor(depth)
+        c = _image_tensor(color)
+        if d is None:
+            d = torch.empty((0, 0, 1), dtype=torch.uint16, device="cuda")
+        if d.dim() == 2:
+            d = d.unsqueeze(-1)
+        if d.dim() != 3 or d.shape[2] != 1:
+            raise RuntimeError(f"Depth image must have one channel, got shape {tuple(d.shape)}")
+        rows, cols = int(d.shape[0]), int(d.shape[1])
+        with_colors = color is not None
+        if c is not None and (c.dim() != 3 or c.shape[2] != 3):
+            raise RuntimeError(f"Color image must have three channels, got shape {tuple(c.shape)}")
+        if with_colors and (rows, cols) != ((0, 0) if c is None else (int(c.shape[0]), int(c.shape[1]))):
+            raise RuntimeError("Depth and color images have different sizes.")
+        cap = (rows // stride) * (cols // stride) if stride >= 1 else 0
+        pts = torch.empty((cap, 3), dtype=torch.float32, device=d.device)
+        col = torch.empty((cap, 3), dtype=torch.float32, device=d.device) if with_colors else None
+        n = C.c_int64(0)
+        check(lib.o3db_unproject(d.data_ptr(), _depth_dtype(d), rows, cols, None if c is None else c.data_ptr(),
+                                 _color_dtype(c), dptr(K), dptr(E), float(depth_scale), float(depth_max), int(stride),
+                                 pts.data_ptr(), None if col is None else col.data_ptr(), C.byref(n),
+                                 current_stream_ptr()))
+        out = PointCloud()
+        out.point["positions"] = pts[: n.value]
+        if with_colors:
+            out.point["colors"] = col[: n.value]
+        return out
+
+    def project_to_depth_image(self, width, height, intrinsics, extrinsics=None, depth_scale=1000.0, depth_max=3.0):
+        """PointCloud::ProjectToDepthImage (PointCloud.cpp:1471-1492): an [height, width, 1] Float32 Image of
+        zc * depth_scale, 0 where no point lands; each pixel keeps the nearest point (see o3db_project).  A cloud
+        without positions gives an empty image, as upstream."""
+        if not self.has_point_positions():
+            return Image(torch.empty((0, 0, 1), dtype=torch.float32))
+        depth, _ = self._project(width, height, intrinsics, extrinsics, depth_scale, depth_max, False)
+        return Image(depth)
+
+    def project_to_rgbd_image(self, width, height, intrinsics, extrinsics=None, depth_scale=1000.0, depth_max=3.0):
+        """PointCloud::ProjectToRGBDImage (PointCloud.cpp:1494-1530): RGBDImage(color [height, width, 3], depth
+        [height, width, 1]), both Float32; the colour of a pixel is that of the point whose depth it keeps."""
+        if not self.has_point_positions():
+            return RGBDImage(Image(torch.empty((0, 0, 1), dtype=torch.float32)),
+                             Image(torch.empty((0, 0, 1), dtype=torch.float32)))
+        if not self.has_point_colors():
+            raise RuntimeError("Unable to project to RGBD without the Color attribute in the point cloud.")
+        depth, color = self._project(width, height, intrinsics, extrinsics, depth_scale, depth_max, True)
+        return RGBDImage(Image(color), Image(depth))
+
+    def _project(self, width, height, intrinsics, extrinsics, depth_scale, depth_max, with_colors):
+        p = self._positions_f32("Project")
+        n = int(p.shape[0])
+        K = _k9(intrinsics)
+        E = as_host_f64_4x4(np.eye(4) if extrinsics is None else extrinsics, "extrinsics")
+        width, height = int(width), int(height)
+        if width < 0 or height < 0:
+            raise RuntimeError(f"Invalid image size {width} x {height}")
+        depth = torch.empty((height, width, 1), dtype=torch.float32, device=p.device)
+        color = cols = None
+        if with_colors:
+            cols = self.point["colors"]
+            if cols.dtype != torch.float32 or cols.dim() != 2 or cols.shape[1] != 3 or cols.shape[0] != n:
+                raise RuntimeError(f"colors must be [{n}, 3] Float32, as the positions (got {tuple(cols.shape)} "
+                                   f"{cols.dtype})")
+            cols = cols.contiguous()
+            color = torch.empty((height, width, 3), dtype=torch.float32, device=p.device)
+        check(lib.o3db_project(p.data_ptr(), None if cols is None else cols.data_ptr(), n, dptr(K), dptr(E),
+                               float(depth_scale), float(depth_max), height, width, depth.data_ptr(),
+                               None if color is None else color.data_ptr(), current_stream_ptr()))
+        return depth, color
+
     def _positions_f32(self, who):
         p = self.point.get("positions")
         if p is None:
