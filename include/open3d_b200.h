@@ -124,6 +124,15 @@ int o3db_compute_pose_colored_icp(const float* source_dev, const float* source_c
                                   double* sums29_dev, double* pose_dev, float* residual_host,
                                   int* inlier_count_host, void* stream);
 
+/* kernel::ComputeRtPointToPoint (kernel/Registration.cpp:365-404; RegistrationCPU.cpp:497-653: Get3x3SxyLinearSystem,
+ * SVD, reflection fix, t = mean(t) - R mean(s)) for a given Int64 correspondence set (-1 = none, n entries, one per
+ * source point).  R_host: row-major 3x3 Float64 rotation, t_host: Float64 translation, inlier_count_host (optional): the
+ * number of valid correspondences.  The sums and the SVD are f64 on the device.  Returns O3DB_ERR_INVALID with upstream's
+ * "No valid correspondence present." when every entry is -1.  When all matches are collinear the rotation is not
+ * unique (upstream's neither): a proper rotation is returned. */
+int o3db_compute_rt_point_to_point(const float* source_dev, const float* target_dev, const int64_t* correspondences_dev,
+                                   int64_t n, double R_host[9], double t_host[3], int* inlier_count_host, void* stream);
+
 /* registration::GetInformationMatrix (registration/Registration.cpp:446-485, pybind get_information_matrix): the 6x6
  * Float64 information matrix GTG of a registration — a clone of the source is transformed, matched to the target by the
  * hybrid search (k = 1), and the Jacobians of the matched TARGET points are reduced
@@ -259,6 +268,14 @@ int o3db_icp_create_colored(const float* source_dev, const float* source_colors_
                             const float* target_colors_dev, const float* target_color_gradients_dev, int64_t m,
                             const double init_source_to_target_host[16], const o3db_icp_options* options,
                             double lambda_geometric, o3db_comm* comm, void* stream, o3db_icp** out);
+/* Same loop for TransformationEstimationPointToPoint (TransformationEstimation.cpp:101-159,
+ * kernel/Registration.cpp:365-404), the estimator registration::ICP uses by default: positions only
+ * (AssertInputMultiScaleICP, Registration.cpp:119-219, asks this estimator for nothing else), no robust kernel
+ * (options->kernel is ignored, the class has none) and no singular-system status.  Search, convergence rule, result
+ * and the iterate / finish / state / reset / destroy calls are those of the point-to-plane handle. */
+int o3db_icp_create_point_to_point(const float* source_dev, int64_t n, const float* target_dev, int64_t m,
+                                   const double init_source_to_target_host[16], const o3db_icp_options* options,
+                                   o3db_comm* comm, void* stream, o3db_icp** out);
 /* Restore the state right after o3db_icp_create (source re-gathered, T = init). */
 int o3db_icp_reset(o3db_icp* icp, void* stream);
 /* Enqueue up to `iterations` ICP iterations (asynchronous, no host sync). */
@@ -280,6 +297,10 @@ int o3db_icp_point_to_plane(const float* source_dev, int64_t n, const float* tar
                             const double init_source_to_target_host[16],
                             const o3db_icp_options* options, o3db_icp_result* result_host,
                             int64_t* correspondences_dev, double* per_iteration_host, void* stream);
+int o3db_icp_point_to_point(const float* source_dev, int64_t n, const float* target_dev, int64_t m,
+                            const double init_source_to_target_host[16], const o3db_icp_options* options,
+                            o3db_icp_result* result_host, int64_t* correspondences_dev, double* per_iteration_host,
+                            void* stream);
 int o3db_icp_colored(const float* source_dev, const float* source_colors_dev, int64_t n, const float* target_dev,
                      const float* target_normals_dev, const float* target_colors_dev,
                      const float* target_color_gradients_dev, int64_t m,

@@ -90,6 +90,10 @@ _SIGS = {
     "o3db_icp_colored": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions), _dbl,
                               C.POINTER(IcpResult), _vp, _dp, _vp]),
     "o3db_icp_create": (_i, [_vp, _i64, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions), _vp, _vp, C.POINTER(_vp)]),
+    "o3db_icp_create_point_to_point": (_i, [_vp, _i64, _vp, _i64, _dp, C.POINTER(IcpOptions), _vp, _vp, C.POINTER(_vp)]),
+    "o3db_icp_point_to_point": (_i, [_vp, _i64, _vp, _i64, _dp, C.POINTER(IcpOptions), C.POINTER(IcpResult), _vp, _dp,
+                                     _vp]),
+    "o3db_compute_rt_point_to_point": (_i, [_vp, _vp, _vp, _i64, _dp, _dp, C.POINTER(_i), _vp]),
     "o3db_get_information_matrix": (_i, [_vp, _i64, _vp, _i64, _dbl, _dp, _dp, _vp]),
     "o3db_compute_information_matrix": (_i, [_vp, _vp, _i64, _dp, _vp, _vp]),
     "o3db_icp_reset": (_i, [_vp, _vp]),

@@ -3,7 +3,8 @@
 // per-block partials -> last block (atomic ticket) sums in block order, with reduce_sums the whole loop of the
 // stand-alone reductions; plus the f64 6x6 solve and pose -> transformation that the reference runs on the host
 // (kernel/TransformationConverter.cpp), and the on-device Gauss-Newton step built from them
-// (gauss_newton_step_warp, left_multiply_warp) that the fused ICP and odometry loops run on one warp.
+// (gauss_newton_step_warp, left_multiply_warp) that the fused ICP and odometry loops run on one warp; and the
+// point-to-point estimator's terms in the same slots with its f64 Kabsch step (kabsch_step_warp).
 #pragma once
 
 #include <utility>
@@ -282,6 +283,177 @@ __device__ __forceinline__ bool gauss_newton_step_warp(const double* sums, doubl
     if (lane == 0) pose_to_T_trig(pose, trig[0], trig[3], trig[1], trig[4], trig[2], trig[5], scratch + 16);
     __syncwarp();
     return true;
+}
+
+// -------------------------------------------------- Kabsch step on one warp (point-to-point)
+
+// Point-to-point slot layout of the 32-wide sum array, about a fixed pivot c (s' = s - c, t' = t - c in f32):
+//   [3 j + k] sum of t'_j s'_k (j, k < 3),  [9 + k] sum of s'_k,  [12 + k] sum of t'_k,  [28] count,  [29] sum of d^2.
+// Raw moments about a fixed point are linear over chunks, shards and ranks, unlike the reference's two-pass centred
+// sums (RegistrationCPU.cpp:497-617), which they reproduce: Sxy = M / n - mean(t') mean(s')^T.
+static constexpr int kP2pSourceSum = 9, kP2pTargetSum = 12, kCountSlot = 28;
+
+template <int NACC>
+__device__ __forceinline__ void accumulate_p2point(float (&acc)[NACC], const float (&s)[3], const float (&t)[3]) {
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) acc[3 * j + k] += t[j] * s[k];
+        acc[kP2pSourceSum + j] += s[j];
+        acc[kP2pTargetSum + j] += t[j];
+    }
+    acc[kCountSlot] += 1.0f;
+}
+
+// One Jacobi rotation of columns P and Q of G (and of V) that makes the two columns of G orthogonal; returns whether
+// it had anything to do.  The indices are template arguments so that both matrices stay in registers.
+template <int P, int Q>
+__device__ __forceinline__ bool jacobi_orthogonalize_columns(double (&G)[3][3], double (&V)[3][3]) {
+    double alpha = 0, beta = 0, gamma = 0;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        alpha += G[r][P] * G[r][P];
+        beta += G[r][Q] * G[r][Q];
+        gamma += G[r][P] * G[r][Q];
+    }
+    if (!(gamma * gamma > 1e-32 * alpha * beta)) return false;   // orthogonal to f64 precision (or a zero column)
+    const double zeta = (beta - alpha) / (2.0 * gamma);
+    const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+    const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        const double gp = G[r][P], gq = G[r][Q], vp = V[r][P], vq = V[r][Q];
+        G[r][P] = c * gp - s * gq;
+        G[r][Q] = s * gp + c * gq;
+        V[r][P] = c * vp - s * vq;
+        V[r][Q] = s * vp + c * vq;
+    }
+    return true;
+}
+
+// The rotation of ComputeRtPointToPointCPU (RegistrationCPU.cpp:619-653): R = U diag(1, 1, sign(det U det V)) V^T for
+// the SVD H = U S V^T of the 3 x 3 row-major H, in f64.  One-sided (Hestenes) Jacobi: plane rotations from the right
+// make the columns of G = H V orthogonal, so that G = U S.  With i, j the two columns of largest norm,
+//   R = u_i v_i^T + u_j v_j^T + (u_i x u_j)(v_i x v_j)^T,
+// which is the formula above whatever the sign of the third singular pair (the two signs cancel against the
+// determinants), so neither the smallest singular value nor its vectors are ever divided by: a planar cloud (rank 2)
+// and a reflection (det H < 0) need no special case.  For rank <= 1 (all matches collinear or coincident) the
+// rotation is not unique, upstream's is whatever LAPACK returns, and this one completes the basis with the coordinate
+// axis least aligned with u_i: a proper rotation with finite entries.
+__device__ inline void kabsch_rotation(const double* H, double* R) {
+    double G[3][3], V[3][3];
+    double scale = 0;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) scale = fmax(scale, fabs(H[k]));
+    const double inv = scale > 0 ? 1.0 / scale : 0.0;   // (the rotation does not depend on the scale of H)
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            G[r][c] = H[3 * r + c] * inv;
+            V[r][c] = r == c ? 1.0 : 0.0;
+        }
+    for (int sweep = 0; sweep < 40; ++sweep) {   // (converges quadratically: 5-8 sweeps in practice)
+        bool any = jacobi_orthogonalize_columns<0, 1>(G, V);
+        any |= jacobi_orthogonalize_columns<0, 2>(G, V);
+        any |= jacobi_orthogonalize_columns<1, 2>(G, V);
+        if (!any) break;
+    }
+    double n2[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) n2[c] = G[0][c] * G[0][c] + G[1][c] * G[1][c] + G[2][c] * G[2][c];
+    // k = the column of smallest norm, (i, j, k) a cyclic shift of (0, 1, 2), then i = the larger of the two
+    const int k = (n2[0] <= n2[1] && n2[0] <= n2[2]) ? 0 : (n2[1] <= n2[2] ? 1 : 2);
+    double gi[3], gj[3], vi[3], vj[3], ni, nj;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        gi[r] = k == 0 ? G[r][1] : (k == 1 ? G[r][2] : G[r][0]);
+        gj[r] = k == 0 ? G[r][2] : (k == 1 ? G[r][0] : G[r][1]);
+        vi[r] = k == 0 ? V[r][1] : (k == 1 ? V[r][2] : V[r][0]);
+        vj[r] = k == 0 ? V[r][2] : (k == 1 ? V[r][0] : V[r][1]);
+    }
+    ni = k == 0 ? n2[1] : (k == 1 ? n2[2] : n2[0]);
+    nj = k == 0 ? n2[2] : (k == 1 ? n2[0] : n2[1]);
+    if (nj > ni) {   // swapping both pairs leaves every term of R as it is
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            double t = gi[r];
+            gi[r] = gj[r];
+            gj[r] = t;
+            t = vi[r];
+            vi[r] = vj[r];
+            vj[r] = t;
+        }
+        const double t = ni;
+        ni = nj;
+        nj = t;
+    }
+    double ui[3], uj[3];
+    if (ni > 0) {
+        const double s = 1.0 / sqrt(ni);
+#pragma unroll
+        for (int r = 0; r < 3; ++r) ui[r] = gi[r] * s;
+    } else {   // H = 0
+        ui[0] = 1.0;
+        ui[1] = ui[2] = 0.0;
+    }
+    if (!(nj > 1e-28 * ni)) {   // rank <= 1: the axis least aligned with u_i
+        const double ax = fabs(ui[0]), ay = fabs(ui[1]), az = fabs(ui[2]);
+        gj[0] = (ax <= ay && ax <= az) ? 1.0 : 0.0;
+        gj[1] = (gj[0] == 0.0 && ay <= az) ? 1.0 : 0.0;
+        gj[2] = (gj[0] == 0.0 && gj[1] == 0.0) ? 1.0 : 0.0;
+    }
+    {   // u_j: the part of g_j orthogonal to u_i, normalised
+        const double d = gj[0] * ui[0] + gj[1] * ui[1] + gj[2] * ui[2];
+#pragma unroll
+        for (int r = 0; r < 3; ++r) uj[r] = gj[r] - d * ui[r];
+        const double s = 1.0 / sqrt(uj[0] * uj[0] + uj[1] * uj[1] + uj[2] * uj[2]);
+#pragma unroll
+        for (int r = 0; r < 3; ++r) uj[r] *= s;
+    }
+    const double uk[3] = {ui[1] * uj[2] - ui[2] * uj[1], ui[2] * uj[0] - ui[0] * uj[2], ui[0] * uj[1] - ui[1] * uj[0]};
+    const double vk[3] = {vi[1] * vj[2] - vi[2] * vj[1], vi[2] * vj[0] - vi[0] * vj[2], vi[0] * vj[1] - vi[1] * vj[0]};
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int c = 0; c < 3; ++c) R[3 * r + c] = ui[r] * vi[c] + uj[r] * vj[c] + uk[r] * vk[c];
+}
+
+// The on-device part of one point-to-point step, with gauss_newton_step_warp's calling convention: ONE warp (all 32
+// lanes must call it), `scratch` the same 64 doubles of shared memory, the update U left in scratch[16, 32).  From the
+// f64 totals in the layout above (sums[28] > 0): the means about the pivot, Sxy, kabsch_rotation, and
+// t = mean(t) - R mean(s) (RegistrationCPU.cpp:651) mapped back from pivot to world coordinates.  There is no
+// singular system for this estimator.  Lane 0 does the arithmetic: it is one dependent chain.
+__device__ __forceinline__ void kabsch_step_warp(const double* sums, const float* pivot, double* scratch) {
+    if ((threadIdx.x & 31) == 0) {
+        const double inv_n = 1.0 / sums[kCountSlot];
+        double ms[3], mt[3], H[9];
+        double* U = scratch + 16;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            ms[k] = sums[kP2pSourceSum + k] * inv_n;
+            mt[k] = sums[kP2pTargetSum + k] * inv_n;
+        }
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+#pragma unroll
+            for (int k = 0; k < 3; ++k) H[3 * j + k] = sums[3 * j + k] * inv_n - mt[j] * ms[k];
+        double* R = scratch;   // (9 doubles; dead once U is written)
+        kabsch_rotation(H, R);
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            double t = mt[j] + (double)pivot[j];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                U[4 * j + k] = R[3 * j + k];
+                t -= R[3 * j + k] * (ms[k] + (double)pivot[k]);
+            }
+            U[4 * j + 3] = t;
+        }
+        U[12] = U[13] = U[14] = 0.0;
+        U[15] = 1.0;
+    }
+    __syncwarp();
 }
 
 // T <- U T for 4 x 4 row-major matrices, by lanes 0-15 of a warp (all sixteen must call it): lane l writes T[l].
