@@ -340,7 +340,7 @@ int o3db_vbg_extract_point_cloud(o3db_vbg* v, float weight_threshold, int64_t ma
     if (rc) return rc;
     ExtractArgs a{};
     a.tab = Table{v->map.table.get(), v->map.nbuckets - 1, v->map.keys.get()};
-    a.size = v->size_dev.get();
+    a.size = &v->status->size;
     a.capacity = (int)v->map.capacity;
     a.res = v->resolution;
     a.res3 = v->resolution * v->resolution * v->resolution;
@@ -370,11 +370,9 @@ int o3db_vbg_extract_point_cloud(o3db_vbg* v, float weight_threshold, int64_t ma
         rc = launch_emit(v, a, ahead, grid, st);
         if (rc) return rc;
     }
-    // the one host synchronisation: the map status (a frame dropped for capacity) and the point count
-    O3DB_CUDA_CHECK(cudaMemcpyAsync(v->h_pinned.get(), v->size_dev.get(), 16 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    // the one host synchronisation (read_status's): the point count and the map status (a frame dropped for capacity)
     O3DB_CUDA_CHECK(cudaMemcpyAsync(v->h_ext_total.get(), v->ext_total.get(), sizeof(long long), cudaMemcpyDeviceToHost, st));
-    O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
-    rc = absorb_status(v, v->h_pinned.get());
+    rc = read_status(v, st);
     if (rc) return rc;
     const long long total = *v->h_ext_total;
     if (total > INT_MAX) {

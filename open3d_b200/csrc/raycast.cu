@@ -329,7 +329,7 @@ static int launch_estimate_range(o3db_vbg* v, const int32_t* coords, int64_t n, 
     a.coords = coords;
     a.keys = v->map.keys.get();
     a.slots = v->frame_slots.get();
-    a.n_dev = coords ? nullptr : v->frame_count;    // block count of the last fused frame
+    a.n_dev = coords ? nullptr : &v->status->frame_count;    // block count of the last fused frame
     a.n = (int)n;
     a.w2c = make_cam(K, E, 1.0f);
     a.h_down = h_down;

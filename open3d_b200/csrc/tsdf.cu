@@ -29,7 +29,6 @@ static constexpr int kT = 256;
 static constexpr int kStepSize = 3;                 // VoxelBlockGridCUDA.cu:125 step_size
 static constexpr int kSamples = kStepSize + 1;      // est_multipler_factor
 static constexpr int kStride = 4;                   // VoxelBlockGrid.cpp:221 down_factor
-static constexpr int kPinnedInts = 16 + 8 * 16;     // o3db_vbg::h_pinned: [0..15] synchronous read-back, then a ring of 8 x 16
 
 __device__ __forceinline__ void mbar_arrive(unsigned long long* b) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory");
@@ -58,7 +57,7 @@ struct TouchArgs {
     int frame_id;
     int* exist_list;         // touched committed slots
     int2* new_list;          // (bucket, candidate) of keys first seen in this frame
-    int* counters;           // [0] n_exist, [1] n_new, [2] overflow flag
+    VbgStatus* status;       // n_exist, n_new, overflow
     int max_list;
 };
 
@@ -121,7 +120,7 @@ __global__ void __launch_bounds__(kT) touch_kernel(TouchArgs a) {
     // only one lane per distinct key and warp gets here)
     const bool first_exist = r >= 0 && a.stamp && atomicExch(&a.stamp[r], a.frame_id) != a.frame_id;
     const bool first_new = r == kResInserted;
-    if (r == kResFull) a.counters[2] = 1;
+    if (r == kResFull) a.status->overflow = 1;
     // warp-aggregated list appends: one atomic per warp and list instead of one per block key
     const unsigned active = __activemask();
     const unsigned me = __ballot_sync(active, first_exist), mn = __ballot_sync(active, first_new);
@@ -129,32 +128,32 @@ __global__ void __launch_bounds__(kT) touch_kernel(TouchArgs a) {
     if (me) {
         const int lead = __ffs(me) - 1;
         int base = 0;
-        if (lane == lead) base = atomicAdd(&a.counters[0], __popc(me));
+        if (lane == lead) base = atomicAdd(&a.status->n_exist, __popc(me));
         base = __shfl_sync(active, base, lead);
         if (first_exist) {
             const int p = base + __popc(me & lt);
             if (p < a.max_list) a.exist_list[p] = r;
-            else a.counters[2] = 1;
+            else a.status->overflow = 1;
         }
     }
     if (mn) {
         const int lead = __ffs(mn) - 1;
         int base = 0;
-        if (lane == lead) base = atomicAdd(&a.counters[1], __popc(mn));
+        if (lane == lead) base = atomicAdd(&a.status->n_new, __popc(mn));
         base = __shfl_sync(active, base, lead);
         if (first_new) {
             const int p = base + __popc(mn & lt);
             if (p < a.max_list) a.new_list[p] = make_int2((int)bucket, cand);
-            else a.counters[2] = 1;
+            else a.status->overflow = 1;
         }
     }
 }
 
 // Stand-alone GetUniqueBlockCoordinates: the winners' keys are the unique set.
-__global__ void emit_unique_keys_kernel(const int2* __restrict__ new_list, const int* __restrict__ counters,
+__global__ void emit_unique_keys_kernel(const int2* __restrict__ new_list, const VbgStatus* __restrict__ status,
                                         const int* __restrict__ cand_keys, int* __restrict__ out, int max_out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int n = min(counters[1], max_out);
+    const int n = min(status->n_new, max_out);
     if (i >= n) return;
     const int* k = cand_keys + 3 * (size_t)new_list[i].y;
     out[3 * i] = k[0];
@@ -172,9 +171,8 @@ struct MapArgs {
     int* buf_indices;
     uint8_t* masks;
     int* bucket_of_input;  // scratch [n]
-    int* size;             // device counter
+    VbgStatus* status;     // size, overflow
     int capacity;
-    int* overflow;
 };
 
 // HashMap::Activate pass 1: claim buckets with provisional markers (candidate id =
@@ -186,7 +184,7 @@ __global__ void activate_claim_kernel(MapArgs a) {
     const int r = probe<true>(a.tab, a.in_keys, i, a.in_keys[3 * i], a.in_keys[3 * i + 1], a.in_keys[3 * i + 2], &bucket);
     a.bucket_of_input[i] = r == kResInserted ? (int)bucket : -1;
     if (a.masks) a.masks[i] = r == kResInserted ? 1 : 0;
-    if (r == kResFull) *a.overflow = 1;
+    if (r == kResFull) a.status->overflow = 1;
 }
 // pass 2: winners pop a slot (CUDAHashBackendBufferAccessor.h:80-83 heap_top), publish key + slot.
 __global__ void activate_commit_kernel(MapArgs a) {
@@ -194,12 +192,12 @@ __global__ void activate_commit_kernel(MapArgs a) {
     if (i >= a.n) return;
     const int b = a.bucket_of_input[i];
     if (b < 0) return;
-    const int slot = atomicAdd(a.size, 1);
+    const int slot = atomicAdd(&a.status->size, 1);
     if (slot >= a.capacity) {
-        atomicSub(a.size, 1);
+        atomicSub(&a.status->size, 1);
         a.tab.table[b] = kTomb;
         if (a.masks) a.masks[i] = 0;
-        *a.overflow = 1;
+        a.status->overflow = 1;
         return;
     }
     a.keys_rw[3 * (size_t)slot] = a.in_keys[3 * i];
@@ -252,23 +250,19 @@ struct IntegrateArgs {
     // list mode
     const int* buf_indices;
     int n_blocks;
-    // fused mode (counters != nullptr): exist_list ++ new_list, commit on the fly
+    // fused mode (status != nullptr): exist_list ++ new_list, commit on the fly
     const int* exist_list;
     const int2* new_list;
     const int* cand_keys;
-    int* counters;           // [0] n_exist [1] n_new [2] overflow [3] ticket
-    int* size;
+    VbgStatus* status;       // the volume's record: read at the start, updated and re-armed by the last CTA
+    VbgStatus* ring;         // pinned host memory, kStatusRing records: the frame's status, written by the last CTA
     int* table;
     int* keys_rw;
     int* stamp;
     int* frame_slots;        // [max] slots of this frame's frustum blocks (Model::frustum_block_coords_)
-    int* frame_count;
-    int* max_new;            // running max of blocks first seen in one frame
-    int* dropped;            // [0] capacity the first dropped frame needed, [1] its frame index + 1 (0 = none)
-    int* host_status;        // pinned host memory, ring of 8 x 16 ints: the frame's status, written by the last CTA
-    int* work;               // fused mode: dynamic work-unit counter (re-armed by the last CTA); null = static striding
-    unsigned long long* exec_ns;   // fused mode: [0] earliest CTA start of this launch (re-armed by the last CTA), [1] sum over
-                                   // launches of (last CTA end - earliest start), [2] launches — %globaltimer, unperturbed by events
+    unsigned long long* exec_ns;   // fused integrate16_kernel only: [0] earliest CTA start of this launch (re-armed by the last
+                                   // CTA), [1] sum over launches of (last CTA end - earliest start), [2] launches — %globaltimer,
+                                   // unperturbed by events
     int frame_id;
     int frame_index;         // 0-based index of the fused frame (reported when a frame is dropped)
     int capacity;
@@ -282,23 +276,112 @@ struct IntegrateArgs {
 };
 
 
+// What every CTA of an integrate launch knows about its frame.  List mode: n_total = n_blocks, nothing else.
+struct Frame {
+    int n_exist, n_new;   // touched committed blocks, keys first seen (fused mode)
+    int size0;            // size before the frame: new block i takes slot size0 + i
+    int n_total;          // blocks to integrate
+    bool drop;
+};
+
+// Start of an integrate launch, after pdl_wait.  Fused mode: ONE decision for every CTA (all the values it reads are
+// final once the touch kernel has finished): a frame whose new blocks do not fit, whose lists overflowed, or that
+// follows a dropped frame, is dropped as a whole — nothing integrated, its provisional table entries released — and
+// reported by the host.
+__device__ __forceinline__ Frame frame_begin(const IntegrateArgs& a) {
+    Frame f{0, 0, 0, a.n_blocks, false};
+    if (!a.status) return f;
+    f.n_exist = a.status->n_exist;
+    f.n_new = a.status->n_new;
+    f.size0 = a.status->size;
+    f.drop = a.status->overflow != 0 || f.size0 + f.n_new > a.capacity;
+    f.n_total = f.drop ? 0 : f.n_exist + f.n_new;
+    if (f.drop) {
+        // no committed key's probe chain passes over a bucket that was empty when the frame began, so emptying every
+        // bucket this frame claimed restores the table exactly
+        const int n_roll = min(f.n_new, a.max_list);
+        for (int i = blockIdx.x * kT + threadIdx.x; i < n_roll; i += gridDim.x * kT) a.table[a.new_list[i].x] = kEmpty;
+    }
+    return f;
+}
+
+// Slot of block b of the launch, and in *key its block coordinate, for work unit `unit` of the block.  Fused mode:
+// the frame's touched committed blocks, then the keys it saw first, which take slots size0, size0 + 1, ...; unit 0 of
+// a new block commits it (key, stamp, table entry), and unit 0 of every block records its slot in frame_slots.
+__device__ __forceinline__ int unit_block(const IntegrateArgs& a, const Frame& f, int b, int unit, const int*& key) {
+    int slot;
+    if (!a.status) {
+        slot = a.buf_indices[b];
+        key = a.block_keys + 3 * (size_t)slot;
+    } else if (b < f.n_exist) {
+        slot = a.exist_list[b];
+        key = a.block_keys + 3 * (size_t)slot;
+    } else {
+        const int2 nl = a.new_list[b - f.n_exist];
+        slot = f.size0 + (b - f.n_exist);
+        key = a.cand_keys + 3 * (size_t)nl.y;
+        if (unit == 0) {
+            a.keys_rw[3 * (size_t)slot] = key[0];
+            a.keys_rw[3 * (size_t)slot + 1] = key[1];
+            a.keys_rw[3 * (size_t)slot + 2] = key[2];
+            a.stamp[slot] = a.frame_id;
+            a.table[nl.x] = slot;
+        }
+    }
+    if (a.status && unit == 0) a.frame_slots[b] = slot;
+    return slot;
+}
+
 // The last CTA of a fused frame publishes the frame's status straight into pinned HOST memory (a posted write over
-// PCIe): slot frame_index & 7 of a ring, sequence tag last.  The host therefore learns sizes without a
+// PCIe): entry frame_index % kStatusRing of the ring, seq last.  The host therefore learns sizes without a
 // device-to-host copy or an event in the stream — the frame's two kernels stay adjacent, which programmatic
 // dependent launch needs.
-__device__ __forceinline__ void publish_status(const IntegrateArgs& a, int size_after, int n_new, int overflow,
-                                               int frame_count, int max_new) {
-    if (!a.host_status) return;
-    volatile int* hs = a.host_status + 16 * (a.frame_index & 7);
-    hs[0] = size_after;
-    hs[5] = n_new;
-    hs[6] = overflow;
-    hs[8] = frame_count;
-    hs[9] = max_new;
-    hs[10] = a.dropped[0];
-    hs[11] = a.dropped[1];
+__device__ __forceinline__ void publish_status(const IntegrateArgs& a, const Frame& f) {
+    volatile VbgStatus* r = a.ring + (a.frame_index & (kStatusRing - 1));
+    r->size = f.drop ? f.size0 : f.size0 + f.n_new;
+    r->n_new = f.n_new;
+    r->overflow = f.drop ? 1 : 0;
+    r->frame_count = f.n_total;
+    r->max_new = a.status->max_new;
+    r->dropped_need = a.status->dropped_need;
+    r->dropped_frame = a.status->dropped_frame;
     __threadfence_system();
-    hs[15] = a.frame_index + 1;
+    r->seq = a.frame_index + 1;
+}
+
+// End of a fused integrate launch: the last CTA to finish updates the status, re-arms the per-frame counters and
+// publishes the frame.
+__device__ __forceinline__ void frame_end(const IntegrateArgs& a, const Frame& f) {
+    __shared__ int s_last;
+    if (!a.status) return;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = atomicAdd(&a.status->ticket, 1) == (int)gridDim.x - 1;
+    __syncthreads();
+    if (!s_last || threadIdx.x != 0) return;
+    VbgStatus* s = a.status;
+    if (f.drop) {
+        if (s->dropped_frame == 0) {          // first dropped frame: what it needed, and which one it was
+            s->dropped_need = f.size0 + f.n_new;
+            s->dropped_frame = a.frame_index + 1;
+        }
+        s->overflow = 1;                      // sticky: later frames are dropped too until the host reserves
+    } else {
+        s->size = f.size0 + f.n_new;
+    }
+    s->frame_count = f.n_total;
+    if (f.n_new > s->max_new) s->max_new = f.n_new;
+    s->n_exist = 0;
+    s->n_new = 0;
+    s->ticket = 0;
+    s->work = 0;
+    if (a.exec_ns) {
+        const unsigned long long now = global_ns();
+        a.exec_ns[1] += now - a.exec_ns[0];
+        a.exec_ns[2] += 1;
+        a.exec_ns[0] = ~0ull;
+    }
+    publish_status(a, f);
 }
 
 // VoxelBlockGridImpl.h:226-303 for one voxel.  Returns false if the voxel is not updated.
@@ -430,55 +513,22 @@ __device__ __forceinline__ void integrate_block_generic(const IntegrateArgs& a, 
 template <typename depth_t, typename color_in_t, bool HAS_COLOR, typename weight_t = uint16_t, typename color_t = uint16_t>
 __global__ void __launch_bounds__(kT) integrate_kernel(IntegrateArgs a) {
     __shared__ int s_slot, s_key[3];
-    const bool fused = a.counters != nullptr;
-    int n_exist = 0, n_new = 0, n_total = a.n_blocks, size0 = 0;
-    bool drop = false;
     pdl_wait();
     pdl_launch_dependents();
-    if (fused) {   // same whole-frame drop rule as integrate16_kernel
-        n_exist = a.counters[0];
-        n_new = a.counters[1];
-        size0 = *a.size;
-        drop = a.counters[2] != 0 || size0 + n_new > a.capacity;
-        n_total = drop ? 0 : n_exist + n_new;
-        if (drop) {
-            const int n_roll = min(n_new, a.max_list);
-            for (int i = blockIdx.x * kT + threadIdx.x; i < n_roll; i += gridDim.x * kT) a.table[a.new_list[i].x] = kEmpty;
-        }
-    }
+    const Frame f = frame_begin(a);
     // work unit = one quarter of a 16^3 block (whole block for other resolutions)
     constexpr bool kVec = sizeof(weight_t) == 2;     // the vectorised quarter-block path is the u16 / u16 layout's
     const int upb = (kVec && a.resolution == 16) ? 4 : 1;
-    for (int wu = blockIdx.x; wu < n_total * upb; wu += gridDim.x) {
+    for (int wu = blockIdx.x; wu < f.n_total * upb; wu += gridDim.x) {
         const int b = wu / upb, unit = wu % upb;
         if (threadIdx.x == 0) {
-            int slot;
             const int* k;
-            if (!fused) {
-                slot = a.buf_indices[b];
-                k = a.block_keys + 3 * (size_t)slot;
-            } else if (b < n_exist) {
-                slot = a.exist_list[b];
-                k = a.block_keys + 3 * (size_t)slot;
-            } else {
-                // a block first seen in this frame: slot = old size + rank; unit 0 commits it
-                const int2 nl = a.new_list[b - n_exist];
-                slot = size0 + (b - n_exist);
-                k = a.cand_keys + 3 * (size_t)nl.y;
-                if (unit == 0) {
-                    a.keys_rw[3 * (size_t)slot] = k[0];
-                    a.keys_rw[3 * (size_t)slot + 1] = k[1];
-                    a.keys_rw[3 * (size_t)slot + 2] = k[2];
-                    a.stamp[slot] = a.frame_id;
-                    a.table[nl.x] = slot;
-                }
-            }
+            const int slot = unit_block(a, f, b, unit, k);
             s_slot = slot;
             if (slot >= 0) {
                 s_key[0] = k[0];
                 s_key[1] = k[1];
                 s_key[2] = k[2];
-                if (fused && unit == 0) a.frame_slots[b] = slot;
             }
         }
         __syncthreads();
@@ -489,33 +539,7 @@ __global__ void __launch_bounds__(kT) integrate_kernel(IntegrateArgs a) {
         }
         __syncthreads();
     }
-    if (fused) {
-        // last CTA publishes the new size and re-arms the per-frame counters
-        __shared__ bool s_last;
-        __threadfence();
-        __syncthreads();
-        if (threadIdx.x == 0) s_last = atomicAdd(&a.counters[3], 1) == (int)gridDim.x - 1;
-        __syncthreads();
-        if (s_last && threadIdx.x == 0) {
-            if (drop) {
-                *a.frame_count = 0;
-                if (a.dropped[1] == 0) {
-                    a.dropped[0] = size0 + n_new;
-                    a.dropped[1] = a.frame_index + 1;
-                }
-                a.counters[2] = 1;
-            } else {
-                *a.frame_count = n_total;
-                *a.size = size0 + n_new;
-            }
-            if (n_new > *a.max_new) *a.max_new = n_new;
-            a.counters[0] = 0;
-            a.counters[1] = 0;
-            a.counters[3] = 0;
-            publish_status(a, drop ? size0 : size0 + n_new, n_new, drop ? 1 : 0, drop ? 0 : n_total, *a.max_new);
-            // counters[2] (overflow) is sticky until the host reads it
-        }
-    }
+    frame_end(a, f);
 }
 
 
@@ -561,7 +585,6 @@ __global__ void __launch_bounds__(kT) integrate16_kernel(const __grid_constant__
     __shared__ int s_meta[2][4];   // slot, block key
     __shared__ int s_rect[4];      // x0, y0 of the staged rectangle, staged?
     __shared__ int s_wu[2];        // work unit of this / the next trip (-1 = none left)
-    __shared__ bool s_last;
     constexpr int kTileCols = kTileRowBytes / (int)sizeof(depth_t);
     const int tid = threadIdx.x;
     if (tid == 0) {
@@ -571,52 +594,12 @@ __global__ void __launch_bounds__(kT) integrate16_kernel(const __grid_constant__
     pdl_wait();                 // the touch kernel's lists / counters, the previous frame's size
     pdl_launch_dependents();
     if (a.exec_ns && tid == 0) atomicMin(&a.exec_ns[0], (unsigned long long)global_ns());
-    const bool fused = a.counters != nullptr;
-    int n_exist = 0, n_new = 0, n_total = a.n_blocks, size0 = 0;
-    bool drop = false;
-    if (fused) {
-        n_exist = a.counters[0];
-        n_new = a.counters[1];
-        size0 = *a.size;
-        // ONE decision for every CTA (all four values are final once the touch kernel has finished): a frame
-        // whose new blocks do not fit, whose lists overflowed, or that follows a dropped frame, is dropped as
-        // a whole — nothing integrated, its provisional table entries released — and reported by the host.
-        drop = a.counters[2] != 0 || size0 + n_new > a.capacity;
-        n_total = drop ? 0 : n_exist + n_new;
-        if (drop) {
-            // no committed key's probe chain passes over a bucket that was empty when the frame began, so
-            // emptying every bucket this frame claimed restores the table exactly
-            const int n_roll = min(n_new, a.max_list);
-            for (int i = blockIdx.x * kT + tid; i < n_roll; i += gridDim.x * kT) a.table[a.new_list[i].x] = kEmpty;
-        }
-    }
-    const int n_units = n_total * 4;
+    const Frame f = frame_begin(a);
+    const int n_units = f.n_total * 4;
 
     auto fetch = [&](int wu, int buf) {    // one thread: metadata of work unit wu
-        const int b = wu >> 2, unit = wu & 3;
-        int slot;
         const int* k;
-        if (!fused) {
-            slot = a.buf_indices[b];
-            k = a.block_keys + 3 * (size_t)slot;
-        } else if (b < n_exist) {
-            slot = a.exist_list[b];
-            k = a.block_keys + 3 * (size_t)slot;
-        } else {
-            // a block first seen in this frame: slot = old size + rank; its unit 0 commits it
-            const int2 nl = a.new_list[b - n_exist];
-            slot = size0 + (b - n_exist);
-            k = a.cand_keys + 3 * (size_t)nl.y;
-            if (unit == 0) {
-                a.keys_rw[3 * (size_t)slot] = k[0];
-                a.keys_rw[3 * (size_t)slot + 1] = k[1];
-                a.keys_rw[3 * (size_t)slot + 2] = k[2];
-                a.stamp[slot] = a.frame_id;
-                a.table[nl.x] = slot;
-            }
-        }
-        if (fused && unit == 0) a.frame_slots[b] = slot;
-        s_meta[buf][0] = slot;
+        s_meta[buf][0] = unit_block(a, f, wu >> 2, wu & 3, k);
         s_meta[buf][1] = k[0];
         s_meta[buf][2] = k[1];
         s_meta[buf][3] = k[2];
@@ -687,7 +670,7 @@ __global__ void __launch_bounds__(kT) integrate16_kernel(const __grid_constant__
                 }
             }
         } else if (tid == 32) {
-            int next = a.work ? (int)gridDim.x + atomicAdd(a.work, 1) : wu + (int)gridDim.x;
+            int next = a.status ? (int)gridDim.x + atomicAdd(&a.status->work, 1) : wu + (int)gridDim.x;
             if (next >= n_units) next = -1;
             s_wu[(it + 1) & 1] = next;
             if (next >= 0) fetch(next, (it + 1) & 1);
@@ -789,38 +772,7 @@ __global__ void __launch_bounds__(kT) integrate16_kernel(const __grid_constant__
             }
         }
     }
-    if (fused) {
-        // last CTA publishes the new size and re-arms the per-frame counters
-        __threadfence();
-        __syncthreads();
-        if (tid == 0) s_last = atomicAdd(&a.counters[3], 1) == (int)gridDim.x - 1;
-        __syncthreads();
-        if (s_last && tid == 0) {
-            if (drop) {
-                *a.frame_count = 0;
-                if (a.dropped[1] == 0) {          // first dropped frame: what it needed, and which one it was
-                    a.dropped[0] = size0 + n_new;
-                    a.dropped[1] = a.frame_index + 1;
-                }
-                a.counters[2] = 1;                // sticky: later frames are dropped too until the host reserves
-            } else {
-                *a.frame_count = n_total;
-                *a.size = size0 + n_new;
-            }
-            if (n_new > *a.max_new) *a.max_new = n_new;
-            a.counters[0] = 0;
-            a.counters[1] = 0;
-            a.counters[3] = 0;
-            if (a.work) *a.work = 0;
-            if (a.exec_ns) {
-                const unsigned long long now = global_ns();
-                a.exec_ns[1] += now - a.exec_ns[0];
-                a.exec_ns[2] += 1;
-                a.exec_ns[0] = ~0ull;
-            }
-            publish_status(a, drop ? size0 : size0 + n_new, n_new, drop ? 1 : 0, drop ? 0 : n_total, *a.max_new);
-        }
-    }
+    frame_end(a, f);
 }
 
 __global__ void inv_weight_table_kernel(float* __restrict__ out) {
@@ -893,6 +845,18 @@ static bool verify_fast_scale(float s) {
         if (fmaf(r, y, q) != d / s) return false;
     }
     return true;
+}
+
+// verify_fast_scale, run once per scale and thread: a sequence of frames keeps its scale, so the 65536-value check is
+// paid once, and each thread keeps its own answer.
+static bool fast_scale_ok(float s) {
+    thread_local float last = 0.f;
+    thread_local bool ok = false;   // == verify_fast_scale(0.f)
+    if (s != last) {
+        last = s;
+        ok = verify_fast_scale(s);
+    }
+    return ok;
 }
 
 // 1 / (w + 1) for every u16 weight: one table per device, built once (and synchronised once), shared by all
@@ -984,7 +948,7 @@ static int grow(o3db_vbg* v, int64_t new_capacity, cudaStream_t st) {
     // new buffers; here slots keep their indices, only the table is rebuilt.
     O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
     int size = 0;
-    O3DB_CUDA_CHECK(cudaMemcpy(&size, v->size_dev.get(), sizeof(int), cudaMemcpyDeviceToHost));
+    O3DB_CUDA_CHECK(cudaMemcpy(&size, &v->status->size, sizeof(int), cudaMemcpyDeviceToHost));
     VbgMap m;
     const int rc = fill_grown_map(v, m, new_capacity, size, st);
     if (rc == O3DB_OK) std::swap(v->map, m);
@@ -992,61 +956,47 @@ static int grow(o3db_vbg* v, int64_t new_capacity, cudaStream_t st) {
     return rc;
 }
 
-int absorb_status(o3db_vbg* v, const int* h) {
-    v->known_size = h[0];
-    v->max_new_seen = std::max<int64_t>(v->max_new_seen, h[9]);
-    if (h[6]) {
+static int absorb_status(o3db_vbg* v, const VbgStatus& s) {
+    v->known_size = s.size;
+    v->max_new_seen = std::max<int64_t>(v->max_new_seen, s.max_new);
+    if (s.overflow) {
         // Frames are atomic and ordered on the device: a frame whose new blocks did not fit (HashMap::Activate would
         // have grown the map, HashMap.cpp:166-181) and every frame after it were dropped whole — nothing integrated,
         // the table restored — so the volume is exactly the state before that frame.
         set_last_error("voxel block hash map capacity (%lld blocks) exceeded: fused frame #%d needed %d blocks; that frame "
                        "and all later ones were dropped (volume unchanged).  Call o3db_vbg_reserve with a larger capacity "
                        "and resubmit from that frame.",
-                       (long long)v->map.capacity, h[11] - 1, h[10]);
+                       (long long)v->map.capacity, s.dropped_frame - 1, s.dropped_need);
         return O3DB_ERR_CAPACITY;
     }
     return O3DB_OK;
 }
 
-// size_dev layout: [0] size, [4] n_exist [5] n_new [6] overflow [7] ticket, [8] frame_count, [9] max_new,
-// [10] blocks the first dropped frame needed, [11] its frame id (0 = no frame dropped)
-static int read_status(o3db_vbg* v, cudaStream_t st) {
-    O3DB_CUDA_CHECK(cudaMemcpyAsync(v->h_pinned.get(), v->size_dev.get(), 16 * sizeof(int), cudaMemcpyDeviceToHost, st));
+// Copies the device status into h_status[0] and waits for it.
+static int copy_status(o3db_vbg* v, cudaStream_t st) {
+    O3DB_CUDA_CHECK(cudaMemcpyAsync(&v->h_status[0], v->status.get(), sizeof(VbgStatus), cudaMemcpyDeviceToHost, st));
     O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
-    return absorb_status(v, v->h_pinned.get());
-}
-
-// Launches the integrate kernel for the input dtypes (VoxelBlockGridCUDA.cu:238-244, value layout u16 weight /
-// u16 colour): the 16^3 fast path with its TMA-staged depth tile, or the generic-resolution kernel.
-template <typename depth_t, typename color_in_t, bool HAS_COLOR>
-static int launch_integrate_typed(IntegrateArgs& a, int depth_dtype, unsigned grid, cudaStream_t st) {
-    if (a.resolution == 16 && a.rows <= 32767 && a.cols <= 65535) {
-        CUtensorMap map;
-        a.use_tile = make_depth_tensor_map(&map, a.depth, depth_dtype, a.rows, a.cols) ? 1 : 0;
-        if (!a.use_tile) memset(&map, 0, sizeof(map));
-        O3DB_CUDA_CHECK(launch_pdl_ex(integrate16_kernel<depth_t, color_in_t, HAS_COLOR>, {grid, kT}, st, a, map));
-    } else {
-        O3DB_CUDA_CHECK(launch_pdl_ex(integrate_kernel<depth_t, color_in_t, HAS_COLOR>, {grid, kT}, st, a));
-    }
     return O3DB_OK;
 }
 
-static int launch_integrate(IntegrateArgs& a, int depth_dtype, int color_dtype, bool has_color, unsigned grid,
-                            cudaStream_t st) {
-    if (depth_dtype == O3DB_DEPTH_U16) {
-        if (!has_color) return launch_integrate_typed<uint16_t, uint8_t, false>(a, depth_dtype, grid, st);
-        if (color_dtype == O3DB_COLOR_U8) return launch_integrate_typed<uint16_t, uint8_t, true>(a, depth_dtype, grid, st);
-        set_last_error("u16 depth requires u8 color (kernel/VoxelBlockGrid.cpp:107-146)");
-        return O3DB_ERR_INVALID;
-    }
-    if (depth_dtype == O3DB_DEPTH_F32) {
-        if (!has_color) return launch_integrate_typed<float, float, false>(a, depth_dtype, grid, st);
-        if (color_dtype == O3DB_COLOR_F32) return launch_integrate_typed<float, float, true>(a, depth_dtype, grid, st);
-        set_last_error("f32 depth requires f32 color (kernel/VoxelBlockGrid.cpp:107-146)");
-        return O3DB_ERR_INVALID;
-    }
-    set_last_error("Unsupported depth dtype");
-    return O3DB_ERR_INVALID;
+int read_status(o3db_vbg* v, cudaStream_t st) {
+    if (int rc = copy_status(v, st)) return rc;
+    return absorb_status(v, v->h_status[0]);
+}
+
+// The status fused frame f published into its ring entry, once the entry's seq says that frame wrote it.  The device
+// writes the entry while the host reads it: every field is read from volatile memory, seq first.
+static bool ring_status(const o3db_vbg* v, int64_t f, VbgStatus& s) {
+    const volatile VbgStatus* e = &v->h_status[1 + (f & (kStatusRing - 1))];
+    if (e->seq != (int)(f + 1)) return false;
+    s.size = e->size;
+    s.n_new = e->n_new;
+    s.overflow = e->overflow;
+    s.frame_count = e->frame_count;
+    s.max_new = e->max_new;
+    s.dropped_need = e->dropped_need;
+    s.dropped_frame = e->dropped_frame;
+    return true;
 }
 
 // Resident CTAs per SM of the integrate kernels (the persistent grids are sized from it).
@@ -1061,12 +1011,49 @@ static unsigned integrate_grid() {
     return (unsigned)(num_sms() * per_sm);
 }
 
-// Arguments common to the handle and the stateless entry points.  checked_scale / checked_scale_ok cache the last
-// verify_fast_scale result.
-static IntegrateArgs base_integrate_args(float voxel_size, int resolution, float& checked_scale, bool& checked_scale_ok,
-                                         const void* depth, const void* color, int color_dtype, int rows, int cols,
-                                         const double* dK, const double* cK, const double* E, float depth_scale,
-                                         float depth_max, float trunc_mult) {
+// Launches the integrate kernel of the input dtypes and value layout (VoxelBlockGridCUDA.cu:238-244).  u16 weight /
+// u16 colour: the 16^3 fast path with its TMA-staged depth tile, or the generic-resolution kernel; f32 weight / f32
+// colour: the generic kernel.  Fused frames take the persistent grid, block lists one CTA per work unit up to it.
+template <typename depth_t, typename color_in_t, bool HAS_COLOR>
+static int launch_integrate_typed(IntegrateArgs& a, int depth_dtype, bool f32_values, cudaStream_t st) {
+    if (f32_values) {
+        const unsigned grid = (unsigned)std::min<int64_t>(a.n_blocks, (int64_t)num_sms() * 8);
+        O3DB_CUDA_CHECK(launch_pdl_ex(integrate_kernel<depth_t, color_in_t, HAS_COLOR, float, float>, {grid, kT}, st, a));
+        return O3DB_OK;
+    }
+    const unsigned grid = a.status ? integrate_grid() : (unsigned)std::min<int64_t>((int64_t)a.n_blocks * 4, integrate_grid());
+    if (a.resolution == 16 && a.rows <= 32767 && a.cols <= 65535) {
+        CUtensorMap map;
+        a.use_tile = make_depth_tensor_map(&map, a.depth, depth_dtype, a.rows, a.cols) ? 1 : 0;
+        if (!a.use_tile) memset(&map, 0, sizeof(map));
+        O3DB_CUDA_CHECK(launch_pdl_ex(integrate16_kernel<depth_t, color_in_t, HAS_COLOR>, {grid, kT}, st, a, map));
+    } else {
+        a.exec_ns = nullptr;   // o3db_vbg_exec_stats times integrate16_kernel only
+        O3DB_CUDA_CHECK(launch_pdl_ex(integrate_kernel<depth_t, color_in_t, HAS_COLOR>, {grid, kT}, st, a));
+    }
+    return O3DB_OK;
+}
+
+// has_color: a.color is set.  Depth dtypes other than u16 / f32 were rejected by check_images.
+static int launch_integrate(IntegrateArgs& a, int depth_dtype, int color_dtype, bool f32_values, cudaStream_t st) {
+    const bool u16 = depth_dtype == O3DB_DEPTH_U16, has_color = a.color != nullptr;
+    if (has_color && color_dtype != (u16 ? O3DB_COLOR_U8 : O3DB_COLOR_F32)) {
+        if (f32_values) set_last_error("Unsupported input data type combination. Expected (float, float) or (uint16, uint8)");
+        else if (u16) set_last_error("u16 depth requires u8 color (kernel/VoxelBlockGrid.cpp:107-146)");
+        else set_last_error("f32 depth requires f32 color (kernel/VoxelBlockGrid.cpp:107-146)");
+        return O3DB_ERR_INVALID;
+    }
+    if (u16)
+        return has_color ? launch_integrate_typed<uint16_t, uint8_t, true>(a, depth_dtype, f32_values, st)
+                         : launch_integrate_typed<uint16_t, uint8_t, false>(a, depth_dtype, f32_values, st);
+    return has_color ? launch_integrate_typed<float, float, true>(a, depth_dtype, f32_values, st)
+                     : launch_integrate_typed<float, float, false>(a, depth_dtype, f32_values, st);
+}
+
+// Arguments common to the handle and the stateless entry points.
+static IntegrateArgs base_integrate_args(float voxel_size, int resolution, const void* depth, const void* color,
+                                         int color_dtype, int rows, int cols, const double* dK, const double* cK,
+                                         const double* E, float depth_scale, float depth_max, float trunc_mult) {
     IntegrateArgs a{};
     a.depth = depth;
     a.color = color;
@@ -1080,11 +1067,7 @@ static IntegrateArgs base_integrate_args(float voxel_size, int resolution, float
     a.depth_max = depth_max;
     a.color_multiplier = color_dtype == O3DB_COLOR_F32 ? 255.0f : 1.0f;   // VoxelBlockGridImpl.h:216-218
     a.resolution = resolution;
-    if (checked_scale != depth_scale) {     // one 65536-value host check per scale (see depth_metres)
-        checked_scale = depth_scale;
-        checked_scale_ok = verify_fast_scale(depth_scale);
-    }
-    a.fast_scale = checked_scale_ok ? 1 : 0;
+    a.fast_scale = fast_scale_ok(depth_scale) ? 1 : 0;
     a.inv_scale = 1.0f / depth_scale;
     // colour intrinsics identical to the depth intrinsics (what slam::Model passes) and sane: interior pixels map to
     // themselves (integrate16_kernel); anything else takes the reference's unproject / project per voxel
@@ -1098,15 +1081,14 @@ static IntegrateArgs base_integrate_args(float voxel_size, int resolution, float
 static IntegrateArgs vbg_integrate_args(o3db_vbg* v, const void* depth, const void* color, int color_dtype, int rows,
                                         int cols, const double* dK, const double* cK, const double* E,
                                         float depth_scale, float depth_max, float trunc_mult) {
-    IntegrateArgs a = base_integrate_args(v->voxel_size, v->resolution, v->checked_scale, v->checked_scale_ok, depth,
-                                          color, color_dtype, rows, cols, dK, cK, E, depth_scale, depth_max, trunc_mult);
+    IntegrateArgs a = base_integrate_args(v->voxel_size, v->resolution, depth, color, color_dtype, rows, cols, dK, cK,
+                                          E, depth_scale, depth_max, trunc_mult);
     a.block_keys = v->map.keys.get();
     a.tsdf = v->map.tsdf.get();
     a.weight = v->map.weight.get();
     a.color_buf = v->map.color.get();
     a.capacity = (int)v->map.capacity;
     a.max_list = (int)v->frustum_cap;
-    a.dropped = v->size_dev.get() + 10;
     a.inv_w = v->inv_w;
     return a;
 }
@@ -1119,8 +1101,9 @@ static int check_images(const void* depth, int depth_dtype, const void* color, i
     return O3DB_OK;
 }
 
-static TouchArgs make_touch_args(o3db_vbg* v, const void* depth, int rows, int cols, const double* K, const double* E,
-                                 float depth_scale, float depth_max, float trunc_mult) {
+// Geometry of a touch launch; the caller adds the table, the lists and the status record.
+static TouchArgs make_touch_args(const void* depth, int rows, int cols, const double* K, const double* E,
+                                 float block_size, float sdf_trunc, float depth_scale, float depth_max) {
     TouchArgs t{};
     double pose[16];
     inverse_transformation(E, pose);               // VoxelBlockGridCUDA.cu:119
@@ -1128,16 +1111,58 @@ static TouchArgs make_touch_args(o3db_vbg* v, const void* depth, int rows, int c
     t.rows = rows;
     t.cols = cols;
     t.cam = make_cam(K, pose, 1.0f);               // :120
-    t.block_size = v->voxel_size * v->resolution;  // :143
-    t.sdf_trunc = v->voxel_size * trunc_mult;      // VoxelBlockGrid.cpp:241
+    t.block_size = block_size;                     // :143
+    t.sdf_trunc = sdf_trunc;
     t.depth_scale = depth_scale;
     t.depth_max = depth_max;
+    return t;
+}
+
+// Touch arguments on the handle's frame scratch.
+static TouchArgs vbg_touch_args(o3db_vbg* v, const void* depth, int rows, int cols, const double* K, const double* E,
+                                float depth_scale, float depth_max, float trunc_mult) {
+    TouchArgs t = make_touch_args(depth, rows, cols, K, E, v->voxel_size * v->resolution,
+                                  v->voxel_size * trunc_mult,   // VoxelBlockGrid.cpp:241
+                                  depth_scale, depth_max);
     t.cand_keys = v->cand_keys.get();
     t.new_list = v->new_list.get();
     t.exist_list = v->exist_list.get();
-    t.counters = v->counters;
+    t.status = v->status.get();
     t.max_list = (int)v->frustum_cap;
     return t;
+}
+
+static int launch_touch(const TouchArgs& t, int depth_dtype, cudaStream_t st) {
+    const int64_t nthreads = (int64_t)(t.rows / kStride) * (t.cols / kStride) * kSamples;
+    const unsigned nb = (unsigned)std::max<int64_t>(1, ceil_div(nthreads, kT));
+    O3DB_CUDA_CHECK(depth_dtype == O3DB_DEPTH_U16 ? launch_pdl_ex(touch_kernel<uint16_t>, {nb, kT}, st, t)
+                                                  : launch_pdl_ex(touch_kernel<float>, {nb, kT}, st, t));
+    return O3DB_OK;
+}
+
+// GetUniqueBlockCoordinates (VoxelBlockGrid.cpp:225-244) on t's frustum table, which only ever holds provisional
+// entries: clears the table and the touch counters, runs the touch kernel and emits the keys it saw first.
+static int unique_block_keys(const TouchArgs& t, int depth_dtype, int32_t* out, int64_t max_out, int64_t* num_host,
+                             cudaStream_t st) {
+    O3DB_CUDA_CHECK(cudaMemsetAsync(t.tab.table, 0xff, ((size_t)t.tab.mask + 1) * sizeof(int), st));   // frustum_hashmap_->Clear()
+    O3DB_CUDA_CHECK(cudaMemsetAsync(&t.status->n_exist, 0, 2 * sizeof(int), st));                        // n_exist, n_new
+    if (int rc = launch_touch(t, depth_dtype, st)) return rc;
+    int n_new = 0;
+    O3DB_CUDA_CHECK(cudaMemcpyAsync(&n_new, &t.status->n_new, sizeof(int), cudaMemcpyDeviceToHost, st));
+    O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
+    const int64_t n = n_new;
+    if (num_host) *num_host = n;
+    if (n == 0) {  // VoxelBlockGridCUDA.cu:193-198
+        set_last_error("No block is touched in TSDF volume, abort integration. Please check specified parameters, "
+                       "especially depth_scale and voxel_size");
+        return O3DB_ERR_NO_BLOCKS;
+    }
+    if (out) {
+        O3DB_REQUIRE(max_out >= n, "block_coords buffer too small: %lld < %lld", (long long)max_out, (long long)n);
+        emit_unique_keys_kernel<<<(unsigned)ceil_div(n, kT), kT, 0, st>>>(t.new_list, t.status, t.cand_keys, out, (int)max_out);
+        O3DB_LAUNCH_CHECK();
+    }
+    return O3DB_OK;
 }
 
 }  // namespace o3db
@@ -1159,18 +1184,14 @@ int o3db_vbg_create(float voxel_size, int block_resolution, int64_t block_count,
     v->resolution = block_resolution;
     v->with_color = with_color != 0;
     if (int rc = alloc_map(v.get(), v->map, block_count, st)) return rc;
-    if (int rc = dev_alloc(v->size_dev, 16, st)) return rc;
-    O3DB_CUDA_CHECK(cudaMemsetAsync(v->size_dev.get(), 0, 16 * sizeof(int), st));
-    v->h_pinned = pinned_block<int[]>(kPinnedInts);
-    if (!v->h_pinned) {
+    if (int rc = dev_alloc(v->status, 1, st)) return rc;
+    O3DB_CUDA_CHECK(cudaMemsetAsync(v->status.get(), 0, sizeof(VbgStatus), st));
+    v->h_status = pinned_block<VbgStatus[]>(1 + kStatusRing);
+    if (!v->h_status) {
         set_last_error("o3db_vbg_create: out of pinned host memory");
         return O3DB_ERR_CUDA;
     }
-    O3DB_CUDA_CHECK(cudaEventCreateWithFlags(&v->ev[0], cudaEventDisableTiming));
-    O3DB_CUDA_CHECK(cudaEventCreateWithFlags(&v->ev[1], cudaEventDisableTiming));
-    v->counters = v->size_dev.get() + 4;
-    v->frame_count = v->size_dev.get() + 8;
-    memset(v->h_pinned.get(), 0, kPinnedInts * sizeof(int));
+    memset(v->h_status.get(), 0, (1 + kStatusRing) * sizeof(VbgStatus));
     if (dev_alloc(v->exec_ns, 3) == O3DB_OK) {   // optional: without it o3db_vbg_exec_stats reports zeros
         const unsigned long long init[3] = {~0ull, 0ull, 0ull};
         cudaMemcpy(v->exec_ns.get(), init, sizeof(init), cudaMemcpyHostToDevice);
@@ -1187,8 +1208,6 @@ int o3db_vbg_create(float voxel_size, int block_resolution, int64_t block_count,
 void o3db_vbg_destroy(o3db_vbg* v) {
     if (!v) return;
     cudaDeviceSynchronize();   // before the buffer owners free with cudaFree
-    for (auto& e : v->ev)
-        if (e) cudaEventDestroy(e);
     for (auto& e : v->prof_ev)
         if (e) cudaEventDestroy(e);
     for (int i = 0; i < 2; ++i) {
@@ -1216,10 +1235,13 @@ int o3db_vbg_reserve(o3db_vbg* v, int64_t capacity, void* stream) {
     // a reserve acknowledges dropped frames (absorb_status): re-arm the device flag and forget the stale
     // read-backs, so that the caller can resubmit from the first dropped frame
     O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
-    O3DB_CUDA_CHECK(cudaMemsetAsync(v->counters + 2, 0, sizeof(int), st));
-    O3DB_CUDA_CHECK(cudaMemsetAsync(v->size_dev.get() + 10, 0, 2 * sizeof(int), st));
-    for (int i = 0; i < kPinnedInts; ++i)
-        if (i % 16 == 6 || i % 16 == 10 || i % 16 == 11) v->h_pinned[i] = 0;
+    VbgStatus* s = v->status.get();
+    for (int* field : {&s->overflow, &s->dropped_need, &s->dropped_frame})
+        O3DB_CUDA_CHECK(cudaMemsetAsync(field, 0, sizeof(int), st));
+    for (int i = 0; i < 1 + kStatusRing; ++i) {
+        VbgStatus& h = v->h_status[i];
+        h.overflow = h.dropped_need = h.dropped_frame = 0;
+    }
     v->sync_next_frame = true;
     return O3DB_OK;
 }
@@ -1261,9 +1283,8 @@ int o3db_vbg_activate(o3db_vbg* v, const int32_t* keys_dev, int64_t n, int32_t* 
     a.buf_indices = buf_indices_dev;
     a.masks = masks_dev;
     a.bucket_of_input = scratch.get();
-    a.size = v->size_dev.get();
+    a.status = v->status.get();
     a.capacity = (int)v->map.capacity;
-    a.overflow = v->counters + 2;
     const unsigned nb = (unsigned)ceil_div(n, kT);
     activate_claim_kernel<<<nb, kT, 0, st>>>(a);
     O3DB_LAUNCH_CHECK();
@@ -1314,36 +1335,12 @@ int o3db_vbg_unique_block_coordinates(o3db_vbg* v, const void* depth_dev, int de
     cudaStream_t st = (cudaStream_t)stream;
     rc = ensure_frame_scratch(v, rows, cols, st);
     if (rc) return rc;
-    // frustum_hashmap_->Clear() (VoxelBlockGrid.cpp:234)
-    O3DB_CUDA_CHECK(cudaMemsetAsync(v->ftable.get(), 0xff, (size_t)v->fbuckets * sizeof(int), st));
-    O3DB_CUDA_CHECK(cudaMemsetAsync(v->counters, 0, 2 * sizeof(int), st));
-    TouchArgs t = make_touch_args(v, depth_dev, rows, cols, K, E, depth_scale, depth_max, trunc_mult);
-    t.tab = Table{v->ftable.get(), v->fbuckets - 1, v->map.keys.get()};
-    t.stamp = nullptr;
-    const int nthreads = (rows / kStride) * (cols / kStride) * kSamples;
-    const unsigned nb = (unsigned)std::max<int64_t>(1, ceil_div(nthreads, kT));
-    if (depth_dtype == O3DB_DEPTH_U16) touch_kernel<uint16_t><<<nb, kT, 0, st>>>(t);
-    else touch_kernel<float><<<nb, kT, 0, st>>>(t);
-    O3DB_LAUNCH_CHECK();
-    int h[2] = {0, 0};
-    O3DB_CUDA_CHECK(cudaMemcpyAsync(h, v->counters, sizeof(h), cudaMemcpyDeviceToHost, st));
-    O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
-    const int64_t n = h[1];
-    if (num_blocks_host) *num_blocks_host = n;
-    if (n == 0) {  // VoxelBlockGridCUDA.cu:193-198
-        set_last_error("No block is touched in TSDF volume, abort integration. Please check specified parameters, "
-                       "especially depth_scale and voxel_size");
-        return O3DB_ERR_NO_BLOCKS;
-    }
-    if (block_coords_dev) {
-        O3DB_REQUIRE(max_blocks >= n, "block_coords buffer too small: %lld < %lld", (long long)max_blocks, (long long)n);
-        emit_unique_keys_kernel<<<(unsigned)ceil_div(n, kT), kT, 0, st>>>(v->new_list.get(), v->counters,
-                                                                          v->cand_keys.get(), block_coords_dev,
-                                                                          (int)max_blocks);
-        O3DB_LAUNCH_CHECK();
-    }
-    O3DB_CUDA_CHECK(cudaMemsetAsync(v->counters, 0, 2 * sizeof(int), st));
-    return O3DB_OK;
+    TouchArgs t = vbg_touch_args(v, depth_dev, rows, cols, K, E, depth_scale, depth_max, trunc_mult);
+    t.tab = Table{v->ftable.get(), v->fbuckets - 1, nullptr};
+    rc = unique_block_keys(t, depth_dtype, block_coords_dev, max_blocks, num_blocks_host, st);
+    // the touch counters are the fused frames' too, and the next frame expects them zero
+    if (rc != O3DB_ERR_CUDA) O3DB_CUDA_CHECK(cudaMemsetAsync(&v->status->n_exist, 0, 2 * sizeof(int), st));
+    return rc;
 }
 
 int o3db_vbg_integrate(o3db_vbg* v, const int32_t* block_coords_dev, int64_t num_blocks, const void* depth_dev,
@@ -1366,8 +1363,7 @@ int o3db_vbg_integrate(o3db_vbg* v, const int32_t* block_coords_dev, int64_t num
                                          E, depth_scale, depth_max, trunc_mult);
     a.buf_indices = buf.get();
     a.n_blocks = (int)num_blocks;
-    const unsigned grid = (unsigned)std::min<int64_t>(num_blocks * 4, (int64_t)integrate_grid());
-    return launch_integrate(a, depth_dtype, color_dtype, has_color, grid, st);
+    return launch_integrate(a, depth_dtype, color_dtype, false, st);
 }
 
 /* Stateless twins of DepthTouchCUDA / IntegrateCUDA for the case where the hash map and its buffers stay the
@@ -1380,58 +1376,28 @@ int o3db_depth_touch(const void* depth_dev, int depth_dtype, int rows, int cols,
     int rc = check_images(depth_dev, depth_dtype, nullptr, 0, rows, cols);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    // scratch of one call: candidate keys, winners, a frustum-sized table (VoxelBlockGrid.cpp:225-234)
+    // scratch of one call: candidate keys, winners, a frustum-sized table (VoxelBlockGrid.cpp:225-234), counters
     const int64_t need = (int64_t)(rows / kStride) * (cols / kStride) * kSamples;
     const unsigned fbuckets = pow2_at_least(2 * need);
-    DevPtr<int> cand, ftable, counters;
+    DevPtr<int> cand, ftable;
     DevPtr<int2> winners;
+    DevPtr<VbgStatus> status;
     rc = dev_alloc(cand, (size_t)need * 3, st);
     if (rc) return rc;
     rc = dev_alloc(winners, (size_t)need, st);
     if (rc) return rc;
     rc = dev_alloc(ftable, fbuckets, st);
     if (rc) return rc;
-    rc = dev_alloc(counters, 4, st);
+    rc = dev_alloc(status, 1, st);
     if (rc) return rc;
-    O3DB_CUDA_CHECK(cudaMemsetAsync(ftable.get(), 0xff, (size_t)fbuckets * sizeof(int), st));
-    O3DB_CUDA_CHECK(cudaMemsetAsync(counters.get(), 0, 4 * sizeof(int), st));
-    TouchArgs t{};
-    double pose[16];
-    inverse_transformation(E, pose);
-    t.depth = depth_dev;
-    t.rows = rows;
-    t.cols = cols;
-    t.cam = make_cam(K, pose, 1.0f);
-    t.block_size = voxel_size * block_resolution;
-    t.sdf_trunc = sdf_trunc;
-    t.depth_scale = depth_scale;
-    t.depth_max = depth_max;
+    TouchArgs t = make_touch_args(depth_dev, rows, cols, K, E, voxel_size * block_resolution, sdf_trunc, depth_scale,
+                                  depth_max);
     t.cand_keys = cand.get();
     t.new_list = winners.get();
-    t.counters = counters.get();
+    t.status = status.get();
     t.max_list = (int)need;
     t.tab = Table{ftable.get(), fbuckets - 1, nullptr};
-    const unsigned nb = (unsigned)std::max<int64_t>(1, ceil_div(need, kT));
-    if (depth_dtype == O3DB_DEPTH_U16) touch_kernel<uint16_t><<<nb, kT, 0, st>>>(t);
-    else touch_kernel<float><<<nb, kT, 0, st>>>(t);
-    O3DB_LAUNCH_CHECK();
-    int h[2] = {0, 0};
-    O3DB_CUDA_CHECK(cudaMemcpyAsync(h, counters.get(), sizeof(h), cudaMemcpyDeviceToHost, st));
-    O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
-    const int64_t n = h[1];
-    if (num_blocks_host) *num_blocks_host = n;
-    if (n == 0) {
-        set_last_error("No block is touched in TSDF volume, abort integration. Please check specified parameters, "
-                       "especially depth_scale and voxel_size");
-        return O3DB_ERR_NO_BLOCKS;
-    }
-    if (block_coords_dev) {
-        O3DB_REQUIRE(max_blocks >= n, "block_coords buffer too small: %lld < %lld", (long long)max_blocks, (long long)n);
-        emit_unique_keys_kernel<<<(unsigned)ceil_div(n, kT), kT, 0, st>>>(winners.get(), counters.get(), cand.get(),
-                                                                          block_coords_dev, (int)max_blocks);
-        O3DB_LAUNCH_CHECK();
-    }
-    return O3DB_OK;
+    return unique_block_keys(t, depth_dtype, block_coords_dev, max_blocks, num_blocks_host, st);
 }
 
 int o3db_integrate_blocks(const void* depth_dev, int depth_dtype, const void* color_dev, int color_dtype, int rows,
@@ -1447,19 +1413,11 @@ int o3db_integrate_blocks(const void* depth_dev, int depth_dtype, const void* co
                  "Unsupported value data type combination. Expected (float, float) or (uint16, uint16)");
     int rc = check_images(depth_dev, depth_dtype, color_dev, color_dtype, rows, cols);
     if (rc) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
     const bool has_color = color_dev != nullptr && color_buf_dev != nullptr;     // VoxelBlockGridImpl.h:202-203
     const float* inv_w = inv_weight_table();
     O3DB_REQUIRE(inv_w != nullptr, "o3db_integrate_blocks: could not build the weight table");
-    static float s_scale = 0.f;   // (benign race: both values are recomputed from depth_scale alone)
-    static bool s_ok = false;
-    float checked_scale = s_scale;
-    bool checked_scale_ok = s_ok;
-    IntegrateArgs a = base_integrate_args(voxel_size, block_resolution, checked_scale, checked_scale_ok, depth_dev,
-                                          has_color ? color_dev : nullptr, color_dtype, rows, cols, dK, cK, E,
-                                          depth_scale, depth_max, 1.0f);
-    s_scale = checked_scale;
-    s_ok = checked_scale_ok;
+    IntegrateArgs a = base_integrate_args(voxel_size, block_resolution, depth_dev, has_color ? color_dev : nullptr,
+                                          color_dtype, rows, cols, dK, cK, E, depth_scale, depth_max, 1.0f);
     a.block_keys = block_keys_dev;
     a.tsdf = tsdf_dev;
     a.weight = (uint16_t*)weight_dev;
@@ -1469,23 +1427,7 @@ int o3db_integrate_blocks(const void* depth_dev, int depth_dtype, const void* co
     a.capacity = INT_MAX;
     a.buf_indices = block_indices_dev;
     a.n_blocks = (int)num_blocks;
-    if (value_layout == O3DB_VALUES_U16) {
-        const unsigned grid = (unsigned)std::min<int64_t>(num_blocks * 4, (int64_t)integrate_grid());
-        return launch_integrate(a, depth_dtype, color_dtype, has_color, grid, st);
-    }
-    // Float32 weight / Float32 colour (VoxelBlockGridCUDA.cu:238-244, second and fourth instantiation)
-    const unsigned grid = (unsigned)std::min<int64_t>(num_blocks, (int64_t)num_sms() * 8);
-    if (depth_dtype == O3DB_DEPTH_U16 && (!has_color || color_dtype == O3DB_COLOR_U8)) {
-        O3DB_CUDA_CHECK(has_color ? launch_pdl_ex(integrate_kernel<uint16_t, uint8_t, true, float, float>, {grid, kT}, st, a)
-                                  : launch_pdl_ex(integrate_kernel<uint16_t, uint8_t, false, float, float>, {grid, kT}, st, a));
-    } else if (depth_dtype == O3DB_DEPTH_F32 && (!has_color || color_dtype == O3DB_COLOR_F32)) {
-        O3DB_CUDA_CHECK(has_color ? launch_pdl_ex(integrate_kernel<float, float, true, float, float>, {grid, kT}, st, a)
-                                  : launch_pdl_ex(integrate_kernel<float, float, false, float, float>, {grid, kT}, st, a));
-    } else {
-        set_last_error("Unsupported input data type combination. Expected (float, float) or (uint16, uint8)");
-        return O3DB_ERR_INVALID;
-    }
-    return O3DB_OK;
+    return launch_integrate(a, depth_dtype, color_dtype, value_layout == O3DB_VALUES_F32, (cudaStream_t)stream);
 }
 
 int o3db_vbg_integrate_frame(o3db_vbg* v, const void* depth_dev, int depth_dtype, const void* color_dev,
@@ -1505,21 +1447,17 @@ int o3db_vbg_integrate_frame(o3db_vbg* v, const void* depth_dev, int depth_dtype
         // the status frame (frames - 2) published into pinned memory; normally long there — the wait only bounds how
         // far the host may run ahead of the device (two frames)
         const int64_t f = v->frames - 2;
-        volatile int* hs = v->h_pinned.get() + 16 + 16 * (int)(f & 7);
-        if (hs[15] != (int)(f + 1)) {
-            const auto t0 = std::chrono::steady_clock::now();
-            while (hs[15] != (int)(f + 1)) {
-                if (std::chrono::steady_clock::now() - t0 > std::chrono::seconds(20)) {
-                    const cudaError_t e = cudaStreamQuery(st);
-                    set_last_error("fused frame #%lld never reported its status (%s)", (long long)f,
-                                   e == cudaSuccess || e == cudaErrorNotReady ? "timeout" : cudaGetErrorString(e));
-                    return O3DB_ERR_CUDA;
-                }
+        VbgStatus s{};
+        const auto t0 = std::chrono::steady_clock::now();
+        while (!ring_status(v, f, s)) {
+            if (std::chrono::steady_clock::now() - t0 > std::chrono::seconds(20)) {
+                const cudaError_t e = cudaStreamQuery(st);
+                set_last_error("fused frame #%lld never reported its status (%s)", (long long)f,
+                               e == cudaSuccess || e == cudaErrorNotReady ? "timeout" : cudaGetErrorString(e));
+                return O3DB_ERR_CUDA;
             }
         }
-        int h[16];
-        for (int i = 0; i < 16; ++i) h[i] = hs[i];
-        rc = absorb_status(v, h);
+        rc = absorb_status(v, s);
         if (rc) return rc;
     }
     const int64_t per_frame = std::max<int64_t>(2 * v->max_new_seen, 2048);
@@ -1532,35 +1470,34 @@ int o3db_vbg_integrate_frame(o3db_vbg* v, const void* depth_dev, int depth_dtype
         }
     }
     const bool has_color = color_dev != nullptr && v->with_color;
-    const int nthreads = (rows / kStride) * (cols / kStride) * kSamples;
-    const unsigned nb = (unsigned)std::max<int64_t>(1, ceil_div(nthreads, kT));
     const bool prof = v->prof_on && (size_t)(3 * v->prof_frames + 2) < v->prof_ev.size();
     if (prof) cudaEventRecord(v->prof_ev[3 * v->prof_frames], st);
     auto touch = [&]() -> int {
         v->frame_id += 1;
-        TouchArgs t = make_touch_args(v, depth_dev, rows, cols, K, E, depth_scale, depth_max, trunc_mult);
+        TouchArgs t = vbg_touch_args(v, depth_dev, rows, cols, K, E, depth_scale, depth_max, trunc_mult);
         t.tab = Table{v->map.table.get(), v->map.nbuckets - 1, v->map.keys.get()};
         t.stamp = v->map.stamp.get();
         t.frame_id = v->frame_id;
-        O3DB_CUDA_CHECK(depth_dtype == O3DB_DEPTH_U16 ? launch_pdl_ex(touch_kernel<uint16_t>, {nb, kT}, st, t)
-                                                      : launch_pdl_ex(touch_kernel<float>, {nb, kT}, st, t));
-        return O3DB_OK;
+        return launch_touch(t, depth_dtype, st);
     };
     rc = touch();
     if (rc) return rc;
     if (v->frames == 0 || v->sync_next_frame) {
         // Nothing is known yet about how many blocks a frame of this sequence adds (first frame, or the first one
         // after a reserve that followed a dropped frame): size the map from the touch kernel's own count before
-        // integrating, as HashMap::Activate does (HashMap.cpp:166-181).  One host synchronisation, once.
+        // integrating, as HashMap::Activate does (HashMap.cpp:166-181).  One host synchronisation, once.  The status
+        // is not absorbed here: a frame whose touch overflowed goes on to the integrate kernel, which drops it and
+        // releases the buckets it claimed.
         v->sync_next_frame = false;
-        O3DB_CUDA_CHECK(cudaMemcpyAsync(v->h_pinned.get(), v->size_dev.get(), 16 * sizeof(int), cudaMemcpyDeviceToHost, st));
-        O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
-        const int64_t need = (int64_t)v->h_pinned[0] + v->h_pinned[5];
-        if (need > v->map.capacity && !v->h_pinned[6]) {
+        rc = copy_status(v, st);
+        if (rc) return rc;
+        const VbgStatus& s = v->h_status[0];
+        const int64_t need = (int64_t)s.size + s.n_new;
+        if (need > v->map.capacity && !s.overflow) {
             rc = grow(v, std::max<int64_t>(2 * v->map.capacity, need + std::max<int64_t>(need / 2, 2048)), st);
             if (rc) return rc;
             // the provisional entries lived in the old table: discover the frame again in the new one
-            O3DB_CUDA_CHECK(cudaMemsetAsync(v->counters, 0, 2 * sizeof(int), st));
+            O3DB_CUDA_CHECK(cudaMemsetAsync(&v->status->n_exist, 0, 2 * sizeof(int), st));
             rc = touch();
             if (rc) return rc;
         }
@@ -1571,20 +1508,16 @@ int o3db_vbg_integrate_frame(o3db_vbg* v, const void* depth_dev, int depth_dtype
     a.exist_list = v->exist_list.get();
     a.new_list = v->new_list.get();
     a.cand_keys = v->cand_keys.get();
-    a.counters = v->counters;
-    a.size = v->size_dev.get();
+    a.status = v->status.get();
+    a.ring = &v->h_status[1];
     a.table = v->map.table.get();
     a.keys_rw = v->map.keys.get();
     a.stamp = v->map.stamp.get();
     a.frame_slots = v->frame_slots.get();
-    a.frame_count = v->frame_count;
-    a.max_new = v->size_dev.get() + 9;
     a.frame_id = v->frame_id;
     a.frame_index = (int)v->frames;
-    a.host_status = v->h_pinned.get() + 16;
-    a.work = v->size_dev.get() + 12;
     a.exec_ns = v->exec_ns.get();
-    rc = launch_integrate(a, depth_dtype, color_dtype, has_color, integrate_grid(), st);
+    rc = launch_integrate(a, depth_dtype, color_dtype, false, st);
     if (rc) return rc;
     if (prof) {
         cudaEventRecord(v->prof_ev[3 * v->prof_frames + 2], st);
@@ -1709,7 +1642,7 @@ int64_t o3db_vbg_last_frustum_blocks(o3db_vbg* v, int32_t* block_coords_dev, int
     cudaStream_t st = (cudaStream_t)stream;
     int rc = read_status(v, st);
     if (rc) return rc;
-    const int64_t n = v->h_pinned[8];
+    const int64_t n = v->h_status[0].frame_count;
     const int64_t m = std::min(n, max_blocks);
     if (m > 0 && block_coords_dev) {
         gather_keys_kernel<<<(unsigned)ceil_div(m, kT), kT, 0, st>>>(v->map.keys.get(), v->frame_slots.get(), (int)m, block_coords_dev);

@@ -2,6 +2,7 @@
 // tsdf.cu (touch / integrate) and raycast.cu (EstimateRange / RayCast).
 #pragma once
 
+#include <cstddef>
 #include <vector>
 
 #include "common.cuh"
@@ -76,6 +77,26 @@ static Cam make_cam(const double* K, const double* E, float scale) {
 template <typename T>
 using GridPtr = DevPtr<T, DeviceFree>;
 
+// Status of a volume.  The handle owns one record on the device; the touch kernel, the integrate kernels and the
+// stand-alone hash ops update it.  The last CTA of fused frame f also publishes it into entry f % kStatusRing of a
+// ring of pinned host records (publish_status), seq last, so that the host can follow the volume without a copy or
+// an event in the stream.
+struct VbgStatus {
+    int size;                          // committed blocks: slots 0 .. size - 1
+    int n_exist, n_new;                // this frame's touched committed blocks and keys first seen (touch_kernel)
+    int overflow;                      // sticky: a list or the table overflowed, or a frame was dropped; cleared by a reserve
+    int ticket;                        // CTAs of the integrate launch that have finished
+    int frame_count;                   // blocks of the last fused frame (frame_slots), 0 if it was dropped
+    int max_new;                       // most keys first seen in one frame
+    int dropped_need, dropped_frame;   // blocks the first dropped frame needed, and its index + 1 (0 = none dropped)
+    int work;                          // dynamic work-unit counter of integrate16_kernel
+    int seq;                           // ring entries only: index + 1 of the frame that wrote the entry
+    int pad[5];
+};
+static_assert(sizeof(VbgStatus) == 64, "VbgStatus is one 64-byte record");
+static_assert(offsetof(VbgStatus, n_new) == offsetof(VbgStatus, n_exist) + sizeof(int), "touch counters are adjacent");
+static constexpr int kStatusRing = 8;   // a power of two
+
 // The hash map and its value buffers, sized together for `capacity` blocks.  A map that grows is built whole beside
 // the old one and swapped in only once it is complete, so that a failed grow leaves the volume as it was.
 struct VbgMap {
@@ -99,19 +120,15 @@ struct o3db_vbg {
     int resolution = 16;
     bool with_color = false;
     o3db::VbgMap map;
-    o3db::GridPtr<int> size_dev;   // [0] size
-    int* counters = nullptr;       // size_dev + 4: [0] n_exist [1] n_new [2] overflow [3] ticket
+    o3db::GridPtr<o3db::VbgStatus> status;
     // per-frame scratch (sized for the frustum capacity (W/4)(H/4)*4)
     int64_t frustum_cap = 0;
     o3db::GridPtr<int> cand_keys;
     o3db::GridPtr<int> exist_list;
     o3db::GridPtr<int2> new_list;
     o3db::GridPtr<int> frame_slots;
-    int* frame_count = nullptr;
     o3db::GridPtr<unsigned long long> exec_ns;   // device-timer statistics of the fused integrate launches (o3db_vbg_exec_stats)
     const float* inv_w = nullptr;  // [65536] 1 / (w + 1) per u16 weight (integrate16_kernel); per-device table, not owned
-    float checked_scale = 0.f;     // depth_scale the 3-FMA u16 division was last verified for ...
-    bool checked_scale_ok = false; // ... and whether it reproduces d / scale for all 65536 u16 values
     bool sync_next_frame = false;  // the next fused frame sizes the map synchronously (after a reserve)
     // frustum-only table for the stand-alone GetUniqueBlockCoordinates
     o3db::GridPtr<int> ftable;
@@ -124,11 +141,9 @@ struct o3db_vbg {
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t copied[2] = {nullptr, nullptr}, consumed[2] = {nullptr, nullptr};
     int64_t host_frames = 0;
-    // host mirrors: size_dev[0..15] is copied to pinned memory after every fused frame
-    // (ring of 2) so that capacity can be managed without a per-frame host sync.
-    o3db::PinnedPtr<int[]> h_pinned; // [0..15] synchronous read-back, then a ring of 8 x 16 ints the device writes into
-                                   // directly (publish_status): per-frame status without a copy or an event in the stream
-    cudaEvent_t ev[2] = {nullptr, nullptr};
+    // [0] synchronous read-back of status (read_status), then the ring the fused frames publish into: capacity is
+    // managed without a per-frame host synchronisation
+    o3db::PinnedPtr<o3db::VbgStatus[]> h_status;
     int frame_id = 0;
     int64_t frames = 0;            // fused frames launched
     int64_t known_size = 0;        // size as last read back (a lower bound)
@@ -152,6 +167,6 @@ struct o3db_vbg {
 };
 
 namespace o3db {
-// tsdf.cu: takes the status words size_dev[0..15] read back into h; O3DB_ERR_CAPACITY after a dropped frame
-int absorb_status(o3db_vbg* v, const int* h);
+// tsdf.cu: reads the status back into h_status[0] (one stream synchronisation); O3DB_ERR_CAPACITY after a dropped frame
+int read_status(o3db_vbg* v, cudaStream_t st);
 }  // namespace o3db
