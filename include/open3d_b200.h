@@ -133,6 +133,29 @@ int o3db_compute_pose_colored_icp(const float* source_dev, const float* source_c
 int o3db_compute_rt_point_to_point(const float* source_dev, const float* target_dev, const int64_t* correspondences_dev,
                                    int64_t n, double R_host[9], double t_host[3], int* inlier_count_host, void* stream);
 
+/* TransformationEstimationSymmetric, for a given Int64 correspondence set (-1 = none, n entries, one per source point;
+ * m target points).  Both clouds need normals ([.,3] f32).  An entry outside [-1, m) returns O3DB_ERR_INVALID with
+ * upstream's "SymmetricICP correspondences must be -1 or a target point index ..." (TransformationEstimation.cpp:85-99).
+ *   o3db_compute_pose_symmetric: kernel::ComputePoseSymmetric (RegistrationCPU.cpp:124-218, RegistrationImpl.h:324-387)
+ *     about the given means (host, the cloud's dtype): the 29 sums of the centred Jacobian [ (s - ms + t - mt) x n ; n ]
+ *     with n = n_t + sign(n_s . n_t) n_s, weights of the objective residual (s - t) . n, [27] its sum of squares, and
+ *     DecodeAndSolve6x6.  Outputs as o3db_compute_pose_point_to_plane's; pose_dev is required.
+ *   o3db_compute_transformation_symmetric: kernel::ComputeTransformationSymmetric (kernel/Registration.cpp:80-135):
+ *     the means of the matched pairs, the pose above and PoseToSymmetricTransformation -> row-major 4x4 Float64 on the
+ *     host; the identity when no entry is valid.  Synchronises the stream.
+ *   o3db_pose_to_symmetric_transformation: PoseToSymmetricTransformation (SymmetricICPImpl.h:19-43), host f64. */
+int o3db_compute_pose_symmetric(const float* source_dev, const float* target_dev, const float* source_normals_dev,
+                                const float* target_normals_dev, const int64_t* correspondences_dev, int64_t n, int64_t m,
+                                const float source_mean_host[3], const float target_mean_host[3],
+                                const o3db_robust_kernel* kernel, double* sums29_dev, double* pose_dev,
+                                float* residual_host, int* inlier_count_host, void* stream);
+int o3db_compute_transformation_symmetric(const float* source_dev, const float* target_dev, const float* source_normals_dev,
+                                          const float* target_normals_dev, const int64_t* correspondences_dev, int64_t n,
+                                          int64_t m, const o3db_robust_kernel* kernel, double transformation_host[16],
+                                          int* inlier_count_host, void* stream);
+void o3db_pose_to_symmetric_transformation(const double pose_host[6], const double source_mean_host[3],
+                                           const double target_mean_host[3], double transformation_host[16]);
+
 /* registration::GetInformationMatrix (registration/Registration.cpp:446-485, pybind get_information_matrix): the 6x6
  * Float64 information matrix GTG of a registration — a clone of the source is transformed, matched to the target by the
  * hybrid search (k = 1), and the Jacobians of the matched TARGET points are reduced
@@ -276,6 +299,13 @@ int o3db_icp_create_colored(const float* source_dev, const float* source_colors_
 int o3db_icp_create_point_to_point(const float* source_dev, int64_t n, const float* target_dev, int64_t m,
                                    const double init_source_to_target_host[16], const o3db_icp_options* options,
                                    o3db_comm* comm, void* stream, o3db_icp** out);
+/* Same loop for TransformationEstimationSymmetric (TransformationEstimation.cpp:229-292, kernel/Registration.cpp:80-135):
+ * both clouds need normals; the working source's normals are rotated with its points every iteration, as
+ * PointCloud::Transform does upstream.  options->kernel is the estimator's robust kernel.  Single GPU only: a
+ * communicator is rejected (O3DB_ERR_INVALID).  Iterate / finish / state / reset / destroy as for the other handles. */
+int o3db_icp_create_symmetric(const float* source_dev, const float* source_normals_dev, int64_t n, const float* target_dev,
+                              const float* target_normals_dev, int64_t m, const double init_source_to_target_host[16],
+                              const o3db_icp_options* options, o3db_comm* comm, void* stream, o3db_icp** out);
 /* Restore the state right after o3db_icp_create (source re-gathered, T = init). */
 int o3db_icp_reset(o3db_icp* icp, void* stream);
 /* Enqueue up to `iterations` ICP iterations (asynchronous, no host sync). */
@@ -301,6 +331,10 @@ int o3db_icp_point_to_point(const float* source_dev, int64_t n, const float* tar
                             const double init_source_to_target_host[16], const o3db_icp_options* options,
                             o3db_icp_result* result_host, int64_t* correspondences_dev, double* per_iteration_host,
                             void* stream);
+int o3db_icp_symmetric(const float* source_dev, const float* source_normals_dev, int64_t n, const float* target_dev,
+                       const float* target_normals_dev, int64_t m, const double init_source_to_target_host[16],
+                       const o3db_icp_options* options, o3db_icp_result* result_host, int64_t* correspondences_dev,
+                       double* per_iteration_host, void* stream);
 int o3db_icp_colored(const float* source_dev, const float* source_colors_dev, int64_t n, const float* target_dev,
                      const float* target_normals_dev, const float* target_colors_dev,
                      const float* target_color_gradients_dev, int64_t m,

@@ -146,6 +146,32 @@ public:
     RobustKernel kernel_;
 };
 
+/// TransformationEstimation.h:214-270: Rusinkiewicz's symmetric objective; both clouds need normals.
+class TransformationEstimationSymmetric {
+public:
+    TransformationEstimationSymmetric() = default;
+    explicit TransformationEstimationSymmetric(const RobustKernel& kernel) : kernel_(kernel) {}
+
+    /// kernel::ComputeTransformationSymmetric (TransformationEstimation.cpp:276-292): the row-major 4x4 Float64
+    /// transformation on the host, the identity without a valid correspondence.  Throws on a correspondence outside
+    /// [-1, target.num_points).
+    std::array<double, 16> ComputeTransformation(const geometry::PointCloud& source, const geometry::PointCloud& target,
+                                                 const int64_t* correspondences_dev, void* stream = nullptr) const {
+        if (!target.HasPointPositions() || !source.HasPointPositions())
+            throw std::runtime_error("Source and/or Target pointcloud is empty.");
+        if (!source.HasPointNormals() || !target.HasPointNormals())
+            throw std::runtime_error("SymmetricICP requires both source and target to have normals.");
+        o3db_robust_kernel k{static_cast<int>(kernel_.type_), kernel_.scaling_parameter_, kernel_.shape_parameter_};
+        std::array<double, 16> T;
+        Check(o3db_compute_transformation_symmetric(source.positions, target.positions, source.normals, target.normals,
+                                                    correspondences_dev, source.num_points, target.num_points, &k, T.data(),
+                                                    nullptr, stream));
+        return T;
+    }
+
+    RobustKernel kernel_;
+};
+
 /// TransformationEstimation.h:318-395 (lambda_geometric outside [0,1] falls back to 0.968, :337-340)
 class TransformationEstimationForColoredICP {
 public:
@@ -268,6 +294,38 @@ inline RegistrationResult ICP(const geometry::PointCloud& source, const geometry
     std::vector<double> per(2 * static_cast<size_t>(criteria.max_iteration_ > 0 ? criteria.max_iteration_ : 1), 0.0);
     Check(o3db_icp_point_to_point(source.positions, source.num_points, target.positions, target.num_points,
                                   init_source_to_target.data(), &opt, &r, correspondences_dev, per.data(), stream));
+    return ToRegistrationResult(r, per, correspondences_dev, callback_after_iteration);
+}
+
+/// registration::ICP for TransformationEstimationSymmetric (and registration_symmetric_icp, Registration.cpp:108-117):
+/// both clouds need normals; the working source's normals turn with its points.
+inline RegistrationResult ICP(const geometry::PointCloud& source, const geometry::PointCloud& target,
+                              double max_correspondence_distance, const std::array<double, 16>& init_source_to_target,
+                              const TransformationEstimationSymmetric& estimation,
+                              const ICPConvergenceCriteria& criteria = ICPConvergenceCriteria(), double voxel_size = -1.0,
+                              const IterationCallback& callback_after_iteration = nullptr,
+                              int64_t* correspondences_dev = nullptr, void* stream = nullptr) {
+    if (!target.HasPointPositions() || !source.HasPointPositions())
+        throw std::runtime_error("Source and/or Target pointcloud is empty.");
+    if (!source.HasPointNormals() || !target.HasPointNormals())
+        throw std::runtime_error("SymmetricICP requires both source and target pointclouds to have normals.");
+    if (max_correspondence_distance <= 0.0)
+        throw std::runtime_error(" Max correspondence distance must be greater than 0, but got " +
+                                 std::to_string(max_correspondence_distance) + " in scale: 0.");
+    if (voxel_size > 0)
+        throw std::runtime_error("voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample)");
+    o3db_icp_options opt{};
+    opt.max_correspondence_distance = max_correspondence_distance;
+    opt.max_iteration = criteria.max_iteration_;
+    opt.relative_fitness = criteria.relative_fitness_;
+    opt.relative_rmse = criteria.relative_rmse_;
+    opt.kernel = {static_cast<int>(estimation.kernel_.type_), estimation.kernel_.scaling_parameter_,
+                  estimation.kernel_.shape_parameter_};
+    o3db_icp_result r{};
+    std::vector<double> per(2 * static_cast<size_t>(criteria.max_iteration_ > 0 ? criteria.max_iteration_ : 1), 0.0);
+    Check(o3db_icp_symmetric(source.positions, source.normals, source.num_points, target.positions, target.normals,
+                             target.num_points, init_source_to_target.data(), &opt, &r, correspondences_dev, per.data(),
+                             stream));
     return ToRegistrationResult(r, per, correspondences_dev, callback_after_iteration);
 }
 

@@ -94,6 +94,15 @@ _SIGS = {
     "o3db_icp_point_to_point": (_i, [_vp, _i64, _vp, _i64, _dp, C.POINTER(IcpOptions), C.POINTER(IcpResult), _vp, _dp,
                                      _vp]),
     "o3db_compute_rt_point_to_point": (_i, [_vp, _vp, _vp, _i64, _dp, _dp, C.POINTER(_i), _vp]),
+    "o3db_compute_pose_symmetric": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, C.POINTER(_f), C.POINTER(_f),
+                                         C.POINTER(RobustKernel), _vp, _vp, C.POINTER(_f), C.POINTER(_i), _vp]),
+    "o3db_compute_transformation_symmetric": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, C.POINTER(RobustKernel), _dp,
+                                                   C.POINTER(_i), _vp]),
+    "o3db_pose_to_symmetric_transformation": (None, [_dp, _dp, _dp, _dp]),
+    "o3db_icp_create_symmetric": (_i, [_vp, _vp, _i64, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions), _vp, _vp,
+                                       C.POINTER(_vp)]),
+    "o3db_icp_symmetric": (_i, [_vp, _vp, _i64, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions), C.POINTER(IcpResult), _vp,
+                                _dp, _vp]),
     "o3db_get_information_matrix": (_i, [_vp, _i64, _vp, _i64, _dbl, _dp, _dp, _vp]),
     "o3db_compute_information_matrix": (_i, [_vp, _vp, _i64, _dp, _vp, _vp]),
     "o3db_icp_reset": (_i, [_vp, _vp]),

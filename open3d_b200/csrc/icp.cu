@@ -1,5 +1,5 @@
 // icp.cu — correspondence search, pose reduction and the fused device-resident
-// ICP loop (point-to-plane, coloured, point-to-point) for sm_90a.  See include/open3d_b200.h for the
+// ICP loop (point-to-plane, coloured, point-to-point, symmetric) for sm_90a.  See include/open3d_b200.h for the
 // reference interfaces each entry point replaces and DESIGN.md for the design.
 //
 // No CPU fallback: every entry point needs a CUDA device.
@@ -150,34 +150,50 @@ static int canonical_ranks(int64_t n, const unsigned* start, const unsigned* key
 // 20 B per point.
 // The original index of a sorted position is not in the record: only the evaluation pass (correspondences) and the
 // ColoredICP set-up read it, so it lives in a separate array (o3db_icp::src_idx) that the iterations never move.
-static constexpr int kSrcChunkBytes = 5 * 32 * 4;
-struct SrcBlocked {
+// The symmetric estimator's record has three more planes, the source normals [nx | ny | nz] (8 planes, 1024 B, 32 B
+// per point): the iteration rotates them with the points.  The plane count is a compile-time constant of each kernel.
+template <int PLANES>
+struct SrcBlockedT {
+    static constexpr int kChunkBytes = PLANES * 32 * 4;
     char* base;
-    __host__ __device__ static size_t bytes(int64_t n_pad) { return (size_t)(n_pad / 32) * kSrcChunkBytes; }
-    __device__ __forceinline__ char* chunk(int i) const { return base + (size_t)(i >> 5) * kSrcChunkBytes; }
+    __host__ __device__ static size_t bytes(int64_t n_pad) { return (size_t)(n_pad / 32) * kChunkBytes; }
+    __device__ __forceinline__ char* chunk(int i) const { return base + (size_t)(i >> 5) * kChunkBytes; }
     // coordinate `axis` (0 = x, 1 = y, 2 = z) of point i
     __device__ __forceinline__ float* coord(int axis, int i) const {
         return reinterpret_cast<float*>(chunk(i) + 128 * axis) + (i & 31);
     }
     __device__ __forceinline__ int* seed(int i) const { return reinterpret_cast<int*>(chunk(i) + 384) + (i & 31); }
     __device__ __forceinline__ float* clearance(int i) const { return reinterpret_cast<float*>(chunk(i) + 512) + (i & 31); }
+    // component `axis` of source normal i (8-plane records only)
+    __device__ __forceinline__ float* normal(int axis, int i) const {
+        static_assert(PLANES == 8, "only the symmetric record carries normals");
+        return reinterpret_cast<float*>(chunk(i) + 640 + 128 * axis) + (i & 31);
+    }
 };
+using SrcBlocked = SrcBlockedT<5>;
+using SrcBlockedSym = SrcBlockedT<8>;
 
-// no seeds, no clearances (and zeroed padding points)
-__global__ void src_blocked_init_kernel(SrcBlocked sb, int64_t n, int64_t n_pad, bool clear_points) {
+// no seeds, no clearances (and zeroed padding points and normals)
+template <int PLANES>
+__global__ void src_blocked_init_kernel(SrcBlockedT<PLANES> sb, int64_t n, int64_t n_pad, bool clear_points) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= n_pad) return;
     *sb.seed((int)i) = -1;
     *sb.clearance((int)i) = 0.f;
-    if (clear_points && i >= n)
+    if (clear_points && i >= n) {
         for (int axis = 0; axis < 3; ++axis) *sb.coord(axis, (int)i) = 0.f;
+        if constexpr (PLANES == 8)
+            for (int axis = 0; axis < 3; ++axis) *sb.normal(axis, (int)i) = 0.f;
+    }
 }
 
-// scatter of the caller's source into the blocked working copy (clone + initial transform); src_idx[sorted position]
-// receives the original index
-__global__ void scatter_source_kernel(const float* __restrict__ pts, int64_t n, Affine T, const unsigned* __restrict__ start,
-                                      const unsigned* __restrict__ key, const unsigned* __restrict__ rank, SrcBlocked sb,
-                                      int* __restrict__ src_idx) {
+// scatter of the caller's source (and, for the 8-plane record, its normals) into the blocked working copy (clone +
+// initial transform, PointCloud::Transform: the normals by the rotation block, transform_normals_kernel's
+// expression); src_idx[sorted position] receives the original index
+template <int PLANES>
+__global__ void scatter_source_kernel(const float* __restrict__ pts, const float* __restrict__ nrm, int64_t n, Affine T,
+                                      const unsigned* __restrict__ start, const unsigned* __restrict__ key,
+                                      const unsigned* __restrict__ rank, SrcBlockedT<PLANES> sb, int* __restrict__ src_idx) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= n) return;
     float x = pts[3 * i], y = pts[3 * i + 1], z = pts[3 * i + 2];
@@ -186,6 +202,12 @@ __global__ void scatter_source_kernel(const float* __restrict__ pts, int64_t n, 
     *sb.coord(0, (int)p) = x;
     *sb.coord(1, (int)p) = y;
     *sb.coord(2, (int)p) = z;
+    if constexpr (PLANES == 8) {
+        const float a = nrm[3 * i], b = nrm[3 * i + 1], c = nrm[3 * i + 2];
+        *sb.normal(0, (int)p) = T.m[0] * a + T.m[1] * b + T.m[2] * c;
+        *sb.normal(1, (int)p) = T.m[4] * a + T.m[5] * b + T.m[6] * c;
+        *sb.normal(2, (int)p) = T.m[8] * a + T.m[9] * b + T.m[10] * c;
+    }
     src_idx[p] = (int)i;
 }
 
@@ -729,6 +751,92 @@ rt_p2point_kernel(const float* __restrict__ src, const float* __restrict__ tgt, 
     if (threadIdx.x == 0) out[16] = s_final[kCountSlot];
 }
 
+struct Vec3f {
+    float v[3];
+};
+
+// ComputePoseSymmetricKernelCPU (RegistrationCPU.cpp:124-180) with GetJacobianSymmetric (RegistrationImpl.h:324-387):
+// the reference's centred Jacobian and residuals about the given means, in f32 op by op in its order; the weight is
+// taken from the objective residual.  Slot 29 counts correspondences outside [-1, m) (the host raises on them).
+template <bool L2LOSS>
+__global__ void __launch_bounds__(kThreads)
+pose_symmetric_kernel(const float* __restrict__ src, const float* __restrict__ tgt, const float* __restrict__ src_n,
+                      const float* __restrict__ tgt_n, const int64_t* __restrict__ corr, int64_t n, int64_t m, Vec3f ms,
+                      Vec3f mt, Robust rk, double* __restrict__ partials, unsigned* ticket, PoseOut out) {
+    __shared__ double s_warp[kThreads / 32][kSumStride];
+    __shared__ double s_final[kSumStride];
+    if (!reduce_sums(n, s_warp, partials, ticket, s_final, [&](int64_t i, float (&acc)[kNumSums]) {
+            const int64_t c = corr[i];
+            if (c == -1) return;
+            if (c < -1 || c >= m) {
+                acc[29] += 1.0f;
+                return;
+            }
+            const float* s = src + 3 * i;
+            const float* t = tgt + 3 * c;
+            const float* ns = src_n + 3 * i;
+            const float* nt = tgt_n + 3 * c;
+            const float dot = __fadd_rn(__fadd_rn(__fmul_rn(ns[0], nt[0]), __fmul_rn(ns[1], nt[1])), __fmul_rn(ns[2], nt[2]));
+            const float sg = dot < 0.f ? -1.f : 1.f;
+            const float nx = __fadd_rn(nt[0], __fmul_rn(sg, ns[0])), ny = __fadd_rn(nt[1], __fmul_rn(sg, ns[1])),
+                        nz = __fadd_rn(nt[2], __fmul_rn(sg, ns[2]));
+            const float sxc = __fsub_rn(s[0], ms.v[0]), syc = __fsub_rn(s[1], ms.v[1]), szc = __fsub_rn(s[2], ms.v[2]);
+            const float txc = __fsub_rn(t[0], mt.v[0]), tyc = __fsub_rn(t[1], mt.v[1]), tzc = __fsub_rn(t[2], mt.v[2]);
+            const float ux = __fadd_rn(sxc, txc), uy = __fadd_rn(syc, tyc), uz = __fadd_rn(szc, tzc);
+            float J[6];
+            J[0] = __fsub_rn(__fmul_rn(uy, nz), __fmul_rn(uz, ny));
+            J[1] = __fsub_rn(__fmul_rn(uz, nx), __fmul_rn(ux, nz));
+            J[2] = __fsub_rn(__fmul_rn(ux, ny), __fmul_rn(uy, nx));
+            J[3] = nx;
+            J[4] = ny;
+            J[5] = nz;
+            const float rc = __fadd_rn(__fadd_rn(__fmul_rn(__fsub_rn(sxc, txc), nx), __fmul_rn(__fsub_rn(syc, tyc), ny)),
+                                       __fmul_rn(__fsub_rn(szc, tzc), nz));
+            const float ro = __fadd_rn(__fadd_rn(__fmul_rn(__fsub_rn(s[0], t[0]), nx), __fmul_rn(__fsub_rn(s[1], t[1]), ny)),
+                                       __fmul_rn(__fsub_rn(s[2], t[2]), nz));
+            const float w = L2LOSS ? 1.0f : robust_weight(rk, ro);
+            int q = 0;
+#pragma unroll
+            for (int j = 0; j < 6; ++j) {
+                const float jw = __fmul_rn(J[j], w);
+#pragma unroll
+                for (int k = 0; k <= j; ++k) acc[q++] += __fmul_rn(jw, J[k]);
+                acc[21 + j] += __fmul_rn(jw, rc);
+            }
+            acc[27] += __fmul_rn(ro, ro);
+            acc[28] += 1.0f;
+        }))
+        return;
+    pose_epilogue(s_final, out);
+}
+
+// The means of the matched pairs (SelectCorrespondingPoints + Mean, kernel/Registration.cpp:86-95) as sums about a
+// pivot inside the target's extent (its first point): out[0, 3) sum of s - p, [3, 6) sum of t - p, [28] count,
+// [29] correspondences outside [-1, m).
+__global__ void __launch_bounds__(kThreads)
+symmetric_means_kernel(const float* __restrict__ src, const float* __restrict__ tgt, const int64_t* __restrict__ corr,
+                       int64_t n, int64_t m, double* __restrict__ partials, unsigned* ticket, double* __restrict__ out) {
+    __shared__ double s_warp[kThreads / 32][kSumStride];
+    __shared__ double s_final[kSumStride];
+    const float p[3] = {__ldg(&tgt[0]), __ldg(&tgt[1]), __ldg(&tgt[2])};
+    if (!reduce_sums(n, s_warp, partials, ticket, s_final, [&](int64_t i, float (&acc)[kNumSums]) {
+            const int64_t c = corr[i];
+            if (c == -1) return;
+            if (c < -1 || c >= m) {
+                acc[29] += 1.0f;
+                return;
+            }
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                acc[k] += src[3 * i + k] - p[k];
+                acc[3 + k] += tgt[3 * c + k] - p[k];
+            }
+            acc[28] += 1.0f;
+        }))
+        return;
+    if (threadIdx.x < kNumSums) out[threadIdx.x] = s_final[threadIdx.x];
+}
+
 // ComputeInformationMatrixKernelCUDA (RegistrationCUDA.cu:492-533) with GetInformationJacobians (RegistrationImpl.h:686-715):
 // the 21 lower-triangle terms of GTG per matched target point (f32, upstream's expression), reduced like the pose sums
 // (f32 per thread over a few terms, then f64: deterministic, and closer to the exact sum than upstream's f32 atomics).
@@ -800,7 +908,10 @@ __global__ void pack_source_intensity_kernel(const int* __restrict__ src_idx, co
 // ------------------------------------------------------------ fused ICP loop
 
 // The estimator of a handle: which per-query terms an iteration adds and which step turns the totals into an update.
-enum : int { kEstPlane = 0, kEstColored = 1, kEstPoint = 2 };
+enum : int { kEstPlane = 0, kEstColored = 1, kEstPoint = 2, kEstSymmetric = 3 };
+// the working source's record of an estimator's kernels (SrcBlockedT)
+template <int EST>
+using SrcOf = SrcBlockedT<EST == kEstSymmetric ? 8 : 5>;
 
 struct IcpState {        // lives in device memory; read back once at the end
     double T[16];        // cumulative source->target transformation (f64)
@@ -846,9 +957,13 @@ struct IcpArgs {
     // multi-GPU, in-kernel exchange (use_peer != 0): every rank's mailbox as mapped into this process
     PeerView peer;
     int use_peer;
-    // point-to-point only: the pivot the moments are taken about (centre of the target's bounding box, world axes)
+    // point-to-point and symmetric: the pivot the moments are taken about (centre of the target's bounding box, world
+    // axes)
     int point_to_point;
     float pivot[3];
+    // symmetric only: the second sum line (sum of s, sum of t; reduce.cuh) per 32-query chunk (8 floats) and per block
+    float* chunk_sums2;
+    double* partials2;
 };
 
 __device__ void set_identity(double* T, float* Uf) {
@@ -868,8 +983,8 @@ static constexpr int kIcpThreads = 768;
 // Host part of DoSingleScaleICPIterations (Registration.cpp:293-358), on device, run by ONE WARP once per
 // iteration (all 32 lanes must call it): gauss_newton_step_warp and left_multiply_warp (reduce.cuh) spread the
 // step over lanes, lane 0 keeps the books.  `s_scratch`: the step's scratch.
-template <bool POINT>
-__device__ void icp_finalize_iteration(const IcpArgs& a, const double* sums, double* s_scratch) {
+template <int EST>
+__device__ void icp_finalize_iteration(const IcpArgs& a, const double* sums, const double* sums2, double* s_scratch) {
     IcpState* st = a.st;
     const int lane = threadIdx.x & 31;
     const double count = sums[28];
@@ -886,9 +1001,11 @@ __device__ void icp_finalize_iteration(const IcpArgs& a, const double* sums, dou
         }
         return;
     }
-    if (POINT) {   // ComputeRtPointToPoint (kernel/Registration.cpp:365-404): no singular case
+    // symmetric: ComputeTransformationSymmetric (kernel/Registration.cpp:80-135)
+    if (EST == kEstPoint) {   // ComputeRtPointToPoint (kernel/Registration.cpp:365-404): no singular case
         kabsch_step_warp(sums, a.pivot, s_scratch);
-    } else if (!gauss_newton_step_warp(sums, s_scratch)) {  // TransformationConverter.cpp:219-225 — the reference raises
+    } else if (EST == kEstSymmetric ? !symmetric_step_warp(sums, sums2, a.pivot, s_scratch)
+                                    : !gauss_newton_step_warp(sums, s_scratch)) {  // TransformationConverter.cpp:219-225 — the reference raises
         if (lane == 0) {
             st->fitness = fitness;
             st->rmse = rmse;
@@ -951,19 +1068,45 @@ __device__ void icp_finalize_evaluate(const IcpArgs& a, const double* sums) {
 // its colour row, fetched by the caller; point-to-point has neither), the estimator's terms + count and sum of d^2,
 // new seed.
 // MODE 0 = iterate, MODE 1 = evaluate (no Jacobian; writes correspondences in the caller's order).
+// The symmetric estimator also rotates the query's source normal `sym->nrm` (stored back like the coordinates) and
+// adds its means terms to the second line `sym->acc2`; `sym` is null for the other estimators.
+struct SymQuery {
+    float nrm[3];
+    float acc2[kSymLine2];
+};
+
+// transform_normals_kernel's expression: the rotation block of the pending update
+__device__ __forceinline__ void rotate_normal(const float* __restrict__ T, float& x, float& y, float& z) {
+    const float a = x, b = y, c = z;
+    x = T[0] * a + T[1] * b + T[2] * c;
+    y = T[4] * a + T[5] * b + T[6] * c;
+    z = T[8] * a + T[9] * b + T[10] * c;
+}
+
 template <bool L2LOSS, int MODE, int EST>
 __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float* s_U, int i, float px, float py, float pz,
                                                   int jp, float clear_prev, const float4* seed_ts, const float4* seed_nn,
-                                                  const float4* seed_cg, float (&acc)[32]) {
+                                                  const float4* seed_cg, float (&acc)[32], SymQuery* sym = nullptr) {
+    const SrcOf<EST> src{a.src.base};
     const float ox = px, oy = py, oz = pz;
     apply_transform(s_U, px, py, pz);
     // Only values whose bits changed are stored back: a store marks its 32-byte sector dirty, and the sector goes back
     // to HBM, even when it rewrites the bits already there.  Once the clouds are aligned, the pending update leaves
     // most coordinates (and with them the clearance) bit-for-bit where they were, and a sector of a plane (8 lanes)
     // whose lanes all skip their store stays clean.
-    if (__float_as_uint(px) != __float_as_uint(ox)) *a.src.coord(0, i) = px;
-    if (__float_as_uint(py) != __float_as_uint(oy)) *a.src.coord(1, i) = py;
-    if (__float_as_uint(pz) != __float_as_uint(oz)) *a.src.coord(2, i) = pz;
+    if (__float_as_uint(px) != __float_as_uint(ox)) *src.coord(0, i) = px;
+    if (__float_as_uint(py) != __float_as_uint(oy)) *src.coord(1, i) = py;
+    if (__float_as_uint(pz) != __float_as_uint(oz)) *src.coord(2, i) = pz;
+    if constexpr (EST == kEstSymmetric) {   // PointCloud::Transform rotates the normals with the points
+        float nx = sym->nrm[0], ny = sym->nrm[1], nz = sym->nrm[2];
+        rotate_normal(s_U, nx, ny, nz);
+        if (__float_as_uint(nx) != __float_as_uint(sym->nrm[0])) *src.normal(0, i) = nx;
+        if (__float_as_uint(ny) != __float_as_uint(sym->nrm[1])) *src.normal(1, i) = ny;
+        if (__float_as_uint(nz) != __float_as_uint(sym->nrm[2])) *src.normal(2, i) = nz;
+        sym->nrm[0] = nx;
+        sym->nrm[1] = ny;
+        sym->nrm[2] = nz;
+    }
     unsigned bj = kNoPoint;
     bool handled = false;
     float clear_new = 0.f;      // what is known about the distance to every point other than the winner
@@ -997,8 +1140,8 @@ __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float*
         bj = nn_search_slow(&a.g, a.tgt, a.cs, px, py, pz, a.r1, a.r1_accept2, a.rr, a.thr, jp);
         clear_new = 0.f;
     }
-    if ((int)bj != jp) *a.src.seed(i) = (int)bj;
-    if (__float_as_uint(clear_new) != __float_as_uint(clear_prev)) *a.src.clearance(i) = clear_new;
+    if ((int)bj != jp) *src.seed(i) = (int)bj;
+    if (__float_as_uint(clear_new) != __float_as_uint(clear_prev)) *src.clearance(i) = clear_new;
     int widx = -1;
     if (bj != kNoPoint) {
         const float4 t = (int)bj == jp ? ts : __ldg(&a.tgt[bj]);   // (just scanned: an L1 hit)
@@ -1018,6 +1161,13 @@ __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float*
                 const float vs[3] = {px, py, pz}, vt[3] = {t.x, t.y, t.z}, nt[3] = {nn.x, nn.y, nn.z};
                 const float dit[3] = {cg.x, cg.y, cg.z};
                 accumulate_colored<L2LOSS, 32>(acc, a.rk, vs, vt, nt, __ldg(&a.sint[i]), cg.w, dit, a.sqrt_lg, a.sqrt_lp);
+            } else if constexpr (EST == kEstSymmetric) {
+                // pivot-relative like point-to-point; the recentring on the means happens once, in the finalize step
+                const float vs[3] = {px - a.pivot[0], py - a.pivot[1], pz - a.pivot[2]};
+                const float vt[3] = {t.x - a.pivot[0], t.y - a.pivot[1], t.z - a.pivot[2]};
+                const float ns[3] = {sym->nrm[0], sym->nrm[1], sym->nrm[2]}, nt[3] = {nn.x, nn.y, nn.z};
+                accumulate_symmetric<L2LOSS>(acc, sym->acc2, vs, vt, ns, nt,
+                                             [&](float r) { return robust_weight(a.rk, r); });
             } else {
                 accumulate_p2plane<L2LOSS, 32>(acc, a.rk, px, py, pz, t.x, t.y, t.z, nn.x, nn.y, nn.z);
             }
@@ -1116,9 +1266,48 @@ __device__ __forceinline__ bool peer_all_reduce(const PeerView& pv, double* s_fi
 
 // Block epilogue of the iteration kernel: block partial -> (last block) grand total, solve, pose update,
 // convergence test.
-template <int MODE, bool POINT>
-__device__ __forceinline__ void icp_block_epilogue(const IcpArgs& a, double (*s_warp)[kSumStride], double* s_final) {
-    if (!block_reduce_to_global<kIcpThreads>(s_warp, a.partials, &a.st->ticket, s_final)) return;
+// The symmetric iteration's second line (acc64b: lane l < 8 holds slot l of the warp's running totals) takes the same
+// route beside it: per-warp slots, a per-block partial in a.partials2 stored before the ticket (block_reduce_to_global's
+// release fence covers it, its acquire fence the loads), and a grand total in block order by warp 0 of the last block.
+template <int MODE, int EST>
+__device__ __forceinline__ void icp_block_epilogue(const IcpArgs& a, double (*s_warp)[kSumStride], double* s_final,
+                                                   double acc64b) {
+    const double* sums2 = nullptr;
+    if constexpr (EST == kEstSymmetric && MODE == 0) {
+        __shared__ double s_warp2[kIcpThreads / 32][kSymLine2];
+        __shared__ double s_final2[kSymLine2];
+        const int lane = threadIdx.x & 31;
+        if (lane < kSymLine2) s_warp2[threadIdx.x >> 5][lane] = acc64b;
+        __syncthreads();
+        if (threadIdx.x < kSymLine2) {
+            double v = 0;
+#pragma unroll
+            for (int w = 0; w < kIcpThreads / 32; ++w) v += s_warp2[w][threadIdx.x];
+            a.partials2[(size_t)blockIdx.x * kSymLine2 + threadIdx.x] = v;
+        }
+        if (!block_reduce_to_global<kIcpThreads>(s_warp, a.partials, &a.st->ticket, s_final)) return;
+        if (threadIdx.x < 32) {   // lane: slot lane & 7 over the blocks lane >> 3, +4, ...; then the four groups
+            constexpr int kU = 8;
+            double v = 0;
+            for (unsigned b = lane >> 3; b < gridDim.x; b += 4 * kU) {
+                double t[kU];
+#pragma unroll
+                for (int u = 0; u < kU; ++u) {
+                    const unsigned bb = b + 4 * u;
+                    t[u] = bb < gridDim.x ? __ldcg(&a.partials2[(size_t)bb * kSymLine2 + (lane & 7)]) : 0.0;
+                }
+#pragma unroll
+                for (int u = 0; u < kU; ++u) v += t[u];
+            }
+            v += __shfl_xor_sync(0xffffffffu, v, 8);
+            v += __shfl_xor_sync(0xffffffffu, v, 16);
+            if (lane < kSymLine2) s_final2[lane] = v;
+            __syncwarp();
+        }
+        sums2 = s_final2;
+    } else {
+        if (!block_reduce_to_global<kIcpThreads>(s_warp, a.partials, &a.st->ticket, s_final)) return;
+    }
     // Every other block has read sums_cached by now.  An iteration has just written or replayed the line of every
     // chunk against the coordinates it left; the evaluation pass moves the coordinates and writes no line.
     if (threadIdx.x == 0) a.st->sums_cached = MODE == 0;
@@ -1131,7 +1320,7 @@ __device__ __forceinline__ void icp_block_epilogue(const IcpArgs& a, double (*s_
                 }
                 return;
             }
-            if (MODE == 0) icp_finalize_iteration<POINT>(a, s_final, &s_warp[0][0]);   // (s_warp is dead: reused as scratch)
+            if (MODE == 0) icp_finalize_iteration<EST>(a, s_final, sums2, &s_warp[0][0]);   // (s_warp is dead: reused as scratch)
             else if (threadIdx.x == 0) icp_finalize_evaluate(a, s_final);
         }
     } else if (threadIdx.x < kNumSums) {
@@ -1163,6 +1352,19 @@ struct __align__(16) IcpStage {
     float4 ts[32];     // the seeds' target points
     float4 ns[EST == kEstPoint ? 1 : 32];     // their normals
     float4 cg[EST == kEstColored ? 32 : 1];   // their colour rows
+};
+// The symmetric stage: its A part is the 8-plane record (SrcBlockedSym), 1024 bytes, still ONE bulk copy.
+template <>
+struct __align__(16) IcpStage<kEstSymmetric> {
+    float px[32];
+    float py[32];
+    float pz[32];
+    int jp[32];
+    float d2[32];
+    float sn[3][32];   // source normals
+    float4 ts[32];
+    float4 ns[32];
+    float4 cg[1];
 };
 
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* b) {
@@ -1227,17 +1429,19 @@ __device__ __forceinline__ void icp_iteration(const IcpArgs& a) {
     const int steps = first < n ? (n - 1 - first) / stride + 1 : 0;
     const int step = s_reverse ? -stride : stride;
     const int start = s_reverse ? first + (steps - 1) * stride : first;
-    constexpr unsigned kBytesA = kSrcChunkBytes;
+    constexpr bool kSym = EST == kEstSymmetric;
+    constexpr unsigned kBytesA = SrcOf<EST>::kChunkBytes;
     static_assert(offsetof(IcpStage<EST>, py) == 128 && offsetof(IcpStage<EST>, pz) == 256 &&
                   offsetof(IcpStage<EST>, jp) == 384 && offsetof(IcpStage<EST>, d2) == 512 &&
                   offsetof(IcpStage<EST>, ts) == kBytesA, "stage A mirrors a chunk record");
+    if constexpr (kSym) static_assert(offsetof(IcpStage<EST>, sn) == 640, "stage A mirrors the symmetric record");
     // chunk c (the warp's c-th step) covers working-source positions [start + c * step, ... + 32)
     auto issue_a = [&](int c) {                // lane 0: ONE TMA bulk copy of chunk c's record into slot c & 1
         if (lane == 0 && c < steps) {
             IcpStage<EST>& sl = sm.stage[w][c & 1];
             unsigned long long* mb = &s_mbar[w][c & 1];
             mbar_arrive_expect_tx(mb, kBytesA);
-            bulk_g2s(sl.px, a.src.chunk(start + c * step), kBytesA, mb);
+            bulk_g2s(sl.px, SrcOf<EST>{a.src.base}.chunk(start + c * step), kBytesA, mb);
         }
     };
     // Sum replay (iterations only).  When the pending update leaves all of a chunk's points bit-for-bit where they
@@ -1247,7 +1451,9 @@ __device__ __forceinline__ void icp_iteration(const IcpArgs& a) {
     // bit, and adding that line to acc64 at the same place in the sweep gives the same totals.  Such a chunk fetches
     // its 128-byte line instead of the seed rows, and does no search, no Jacobian, no reduction and no store.  Its
     // seeds already hold the winners; only a clearance that a search would have re-established stays as it was,
-    // which can send a later search down another (equally exact) path.
+    // which can send a later search down another (equally exact) path.  The symmetric estimator's terms also read the
+    // source normals, so its chunks replay only when the update leaves those bit-for-bit unchanged as well, and a
+    // replayed chunk fetches its 32-byte second line with the first.
     bool replay_b = false;   // the decision of the last issue_b, warp-uniform
     auto issue_b = [&](int c) {                // every lane: gather its seed's rows of chunk c (needs A(c))
         if (c < steps) {
@@ -1261,11 +1467,22 @@ __device__ __forceinline__ void icp_iteration(const IcpArgs& a) {
                 apply_transform(s_U, x, y, z);   // the expression icp_process_query applies
                 unchanged = __float_as_uint(x) == __float_as_uint(ox) && __float_as_uint(y) == __float_as_uint(oy) &&
                             __float_as_uint(z) == __float_as_uint(oz);
+                if constexpr (kSym) {
+                    float nx = sl.sn[0][lane], ny = sl.sn[1][lane], nz = sl.sn[2][lane];
+                    rotate_normal(s_U, nx, ny, nz);   // the expression icp_process_query applies
+                    unchanged = unchanged && __float_as_uint(nx) == __float_as_uint(sl.sn[0][lane]) &&
+                                __float_as_uint(ny) == __float_as_uint(sl.sn[1][lane]) &&
+                                __float_as_uint(nz) == __float_as_uint(sl.sn[2][lane]);
+                }
             }
             replay_b = MODE == 0 && s_cached && __all_sync(0xffffffffu, unchanged);
             if (replay_b) {
                 if (lane < 8)
                     cp_async16_cg(&sl.ts[lane], reinterpret_cast<const float4*>(a.chunk_sums + q0) + lane);
+                if constexpr (kSym)   // ts[8, 10): the chunk's second line
+                    if (lane >= 8 && lane < 8 + kSymLine2 / 4)
+                        cp_async16_cg(&sl.ts[lane],
+                                      reinterpret_cast<const float4*>(a.chunk_sums2 + (q0 >> 5) * kSymLine2) + (lane - 8));
             } else {
                 const int jp = sl.jp[lane];
                 if (jp >= 0) {
@@ -1279,6 +1496,7 @@ __device__ __forceinline__ void icp_iteration(const IcpArgs& a) {
     };
 
     double acc64 = 0.0;      // lane l: running total of slot l over this warp's queries
+    double acc64b = 0.0;     // symmetric, lane l < 8: running total of slot l of the second line
     issue_a(0);
     issue_a(1);
     issue_b(0);
@@ -1291,12 +1509,19 @@ __device__ __forceinline__ void icp_iteration(const IcpArgs& a) {
         const float px = sl.px[lane], py = sl.py[lane], pz = sl.pz[lane];
         const int jp = sl.jp[lane];
         const float clear_prev = sl.d2[lane];
+        SymQuery sym;
+        if constexpr (kSym) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) sym.nrm[k] = sl.sn[k][lane];
+        }
         __syncwarp();          // every lane has read its point / jp / d2 of slot c & 1: hand that part back to the producer
         issue_a(c + 2);
         issue_b(c + 1);
         // (ts / ns / cg of slot c & 1 are rewritten by issue_b(c + 2), i.e. in the NEXT trip: still valid below)
         if (replay) {
             acc64 += (double)reinterpret_cast<const float*>(sl.ts)[lane];
+            if constexpr (kSym)
+                if (lane < kSymLine2) acc64b += (double)reinterpret_cast<const float*>(sl.ts)[32 + lane];
             continue;
         }
         const int i = q0 + lane;
@@ -1304,15 +1529,27 @@ __device__ __forceinline__ void icp_iteration(const IcpArgs& a) {
 #pragma unroll
         for (int k = 0; k < 32; ++k) term[k] = 0.f;
         bool matched = false;
+        if constexpr (kSym) {
+#pragma unroll
+            for (int k = 0; k < kSymLine2; ++k) sym.acc2[k] = 0.f;
+        }
         if (i < n)
             matched = icp_process_query<L2LOSS, MODE, EST>(a, s_U, i, px, py, pz, jp, clear_prev, &sl.ts[lane],
                                                            &sl.ns[EST == kEstPoint ? 0 : lane],
-                                                           &sl.cg[EST == kEstColored ? lane : 0], term);
+                                                           &sl.cg[EST == kEstColored ? lane : 0], term, &sym);
         const float line = icp_accumulate_chunk(term, matched, acc64);
         if (MODE == 0) a.chunk_sums[q0 + lane] = line;   // one coalesced 128-byte store
+        if constexpr (kSym && MODE == 0) {   // the second line: same rules (+0.0 when no lane matched)
+            float line2 = 0.f;
+            if (__any_sync(0xffffffffu, matched)) {
+                line2 = warp_transpose_sum8(sym.acc2);
+                acc64b += (double)line2;
+            }
+            if (lane < kSymLine2) a.chunk_sums2[(q0 >> 5) * kSymLine2 + lane] = line2;
+        }
     }
     if (lane < kNumSums) s_warp[w][lane] = acc64;
-    icp_block_epilogue<MODE, EST == kEstPoint>(a, s_warp, s_final);
+    icp_block_epilogue<MODE, EST>(a, s_warp, s_final, acc64b);
 }
 
 template <bool L2LOSS, int MODE, bool COLORED = false>
@@ -1328,14 +1565,22 @@ icp_point_iteration_kernel(const __grid_constant__ IcpArgs a) {
     icp_iteration<true, 0, kEstPoint>(a);
 }
 
-// Multi-GPU: runs after the all-reduce of st->sums.
+// The symmetric iteration and its evaluation pass.  The evaluation pass is not icp_iteration_kernel<true, 1>: it reads
+// and moves the 8-plane record, whose stride is a compile-time constant of the kernel.
+template <bool L2LOSS, int MODE>
+__global__ void __launch_bounds__(kIcpThreads, 1)
+icp_symmetric_iteration_kernel(const __grid_constant__ IcpArgs a) {
+    icp_iteration<L2LOSS, MODE, kEstSymmetric>(a);
+}
+
+// Multi-GPU: runs after the all-reduce of st->sums.  (Symmetric handles take no communicator.)
 template <int MODE>
 __global__ void icp_finalize_kernel(IcpArgs a) {   // <<<1, 32>>>
     __shared__ double s_scratch[64];
     if (MODE == 0) {
         if (a.st->done) return;
-        if (a.point_to_point) icp_finalize_iteration<true>(a, a.st->sums, s_scratch);
-        else icp_finalize_iteration<false>(a, a.st->sums, s_scratch);
+        if (a.point_to_point) icp_finalize_iteration<kEstPoint>(a, a.st->sums, nullptr, s_scratch);
+        else icp_finalize_iteration<kEstPlane>(a, a.st->sums, nullptr, s_scratch);
     } else if (threadIdx.x == 0) {
         icp_finalize_evaluate(a, a.st->sums);
     }
@@ -1379,6 +1624,11 @@ struct o3db_icp {
     // TransformationEstimationPointToPoint: no target normals (nns.nrm4 stays null), no robust kernel
     bool point = false;
     float pivot[3] = {0.f, 0.f, 0.f};
+    // TransformationEstimationSymmetric: 8-plane records carrying the source normals, and the second sum line
+    bool symmetric = false;
+    const float* src_normals_user = nullptr;
+    o3db::DevPtr<float> chunk_sums2;    // n_pad / 4 floats: 8 per 32-query chunk
+    o3db::DevPtr<double> partials2;     // grid_blocks x 8
 };
 
 namespace o3db {
@@ -1386,6 +1636,9 @@ namespace o3db {
 typedef void (*IcpKernel)(IcpArgs);
 // mode 0 = iterate (loss / colour of the handle), 1 = final evaluation (no Jacobian)
 static IcpKernel icp_kernel_for(const o3db_icp* c, int mode) {
+    if (c->symmetric)
+        return mode == 1 ? icp_symmetric_iteration_kernel<true, 1>
+                         : c->l2loss ? icp_symmetric_iteration_kernel<true, 0> : icp_symmetric_iteration_kernel<false, 0>;
     if (mode == 1) return icp_iteration_kernel<true, 1, false>;
     if (c->point) return icp_point_iteration_kernel;
     if (c->colored) return c->l2loss ? icp_iteration_kernel<true, 0, true> : icp_iteration_kernel<false, 0, true>;
@@ -1394,6 +1647,7 @@ static IcpKernel icp_kernel_for(const o3db_icp* c, int mode) {
 
 // dynamic shared memory of the handle's iteration kernels (the stage ring)
 static size_t icp_smem_bytes(const o3db_icp* c, int mode) {
+    if (c->symmetric) return sizeof(IcpStagedSmem<kEstSymmetric>);
     if (mode == 1) return sizeof(IcpStagedSmem<kEstPlane>);
     return c->colored ? sizeof(IcpStagedSmem<kEstColored>) : c->point ? sizeof(IcpStagedSmem<kEstPoint>) : sizeof(IcpStagedSmem<kEstPlane>);
 }
@@ -1440,6 +1694,8 @@ static IcpArgs make_args(o3db_icp* c) {
     a.sqrt_lp = (float)sqrt(1.0 - c->lambda_geometric);
     a.point_to_point = c->point ? 1 : 0;
     for (int k = 0; k < 3; ++k) a.pivot[k] = c->pivot[k];
+    a.chunk_sums2 = c->chunk_sums2.get();
+    a.partials2 = c->partials2.get();
     return a;
 }
 
@@ -1451,8 +1707,12 @@ static int icp_init_state(o3db_icp* c, cudaStream_t st) {
     }
     memcpy(c->h_st.get(), &h, sizeof(h));
     O3DB_CUDA_CHECK(cudaMemcpyAsync(c->st.get(), c->h_st.get(), sizeof(IcpState), cudaMemcpyHostToDevice, st));
-    src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlocked{c->src_blk.get()}, c->n, c->n_pad,
-                                                                                         false);   // no seeds, no clearances
+    const unsigned nb = (unsigned)ceil_div(c->n_pad, kThreads);
+    if (c->symmetric)
+        src_blocked_init_kernel<<<nb, kThreads, 0, st>>>(SrcBlockedSym{c->src_blk.get()}, c->n, c->n_pad, false);
+    else
+        src_blocked_init_kernel<<<nb, kThreads, 0, st>>>(SrcBlocked{c->src_blk.get()}, c->n, c->n_pad,
+                                                         false);   // no seeds, no clearances
     O3DB_LAUNCH_CHECK();
     c->launched = 0;
     return O3DB_OK;
@@ -1462,9 +1722,14 @@ static int icp_gather_source(o3db_icp* c, cudaStream_t st) {
     Affine T0;
     for (int i = 0; i < 16; ++i) T0.m[i] = (float)c->init_T[i];   // Transform.cpp:29-31: T cast to the point dtype
     if (c->n == 0) return O3DB_OK;
-    scatter_source_kernel<<<(unsigned)ceil_div(c->n, kThreads), kThreads, 0, st>>>(c->src_user, c->n, T0, c->src_start.get(),
-                                                                                  c->src_key.get(), c->src_rank.get(),
-                                                                                  SrcBlocked{c->src_blk.get()}, c->src_idx.get());
+    const unsigned nb = (unsigned)ceil_div(c->n, kThreads);
+    if (c->symmetric)
+        scatter_source_kernel<<<nb, kThreads, 0, st>>>(c->src_user, c->src_normals_user, c->n, T0, c->src_start.get(),
+                                                       c->src_key.get(), c->src_rank.get(), SrcBlockedSym{c->src_blk.get()},
+                                                       c->src_idx.get());
+    else
+        scatter_source_kernel<<<nb, kThreads, 0, st>>>(c->src_user, nullptr, c->n, T0, c->src_start.get(), c->src_key.get(),
+                                                       c->src_rank.get(), SrcBlocked{c->src_blk.get()}, c->src_idx.get());
     O3DB_LAUNCH_CHECK();
     return O3DB_OK;
 }
@@ -1706,6 +1971,127 @@ int o3db_compute_rt_point_to_point(const float* source_dev, const float* target_
     return O3DB_OK;
 }
 
+}  // extern "C"
+
+namespace o3db {
+
+static constexpr const char* kSymCorrMessage =
+        "SymmetricICP correspondences must be -1 or a target point index in [0, %lld), but an out-of-range value was found.";
+
+// pose_symmetric_kernel over the given means; with `h` the sums read back (synchronises the stream).
+static int symmetric_pose_sums(const float* src, const float* tgt, const float* src_n, const float* tgt_n,
+                               const int64_t* corr, int64_t n, int64_t m, const Vec3f& ms, const Vec3f& mt,
+                               const o3db_robust_kernel* kernel, double* pose_dev, double (&h)[kSumStride], int* status,
+                               cudaStream_t st) {
+    PoseScratch s;
+    if (int rc = pose_scratch_alloc(&s, n, st)) return rc;
+    const Robust rk{kernel ? kernel->method : 0, kernel ? (float)kernel->scale : 1.f, kernel ? kernel->shape : 1.0};
+    (rk.method == O3DB_ROBUST_L2 ? pose_symmetric_kernel<true> : pose_symmetric_kernel<false>)<<<s.blocks, kThreads, 0, st>>>(
+            src, tgt, src_n, tgt_n, corr, n, m, ms, mt, rk, s.partials, s.ticket, PoseOut{s.sums, pose_dev, s.status});
+    O3DB_LAUNCH_CHECK();
+    O3DB_CUDA_CHECK(cudaMemcpyAsync(h, s.sums, sizeof(h), cudaMemcpyDeviceToHost, st));
+    O3DB_CUDA_CHECK(cudaMemcpyAsync(status, s.status, sizeof(int), cudaMemcpyDeviceToHost, st));
+    O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
+    if (h[29] > 0) {
+        set_last_error(kSymCorrMessage, (long long)m);
+        return O3DB_ERR_INVALID;
+    }
+    return O3DB_OK;
+}
+
+}  // namespace o3db
+
+extern "C" {
+
+int o3db_compute_pose_symmetric(const float* source_dev, const float* target_dev, const float* source_normals_dev,
+                                const float* target_normals_dev, const int64_t* correspondences_dev, int64_t n, int64_t m,
+                                const float source_mean[3], const float target_mean[3], const o3db_robust_kernel* kernel,
+                                double* sums29_dev, double* pose_dev, float* residual_host, int* inlier_count_host,
+                                void* stream) {
+    O3DB_REQUIRE(n > 0 && m > 0 && source_dev && target_dev && source_normals_dev && target_normals_dev &&
+                         correspondences_dev && source_mean && target_mean && pose_dev,
+                 "o3db_compute_pose_symmetric: bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    const Vec3f ms{{source_mean[0], source_mean[1], source_mean[2]}}, mt{{target_mean[0], target_mean[1], target_mean[2]}};
+    double h[kSumStride];
+    int status = 0;
+    int rc = symmetric_pose_sums(source_dev, target_dev, source_normals_dev, target_normals_dev, correspondences_dev, n, m,
+                                 ms, mt, kernel, pose_dev, h, &status, st);
+    if (rc) return rc;
+    if (sums29_dev) {
+        O3DB_CUDA_CHECK(cudaMemcpyAsync(sums29_dev, h, 29 * sizeof(double), cudaMemcpyHostToDevice, st));
+        O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
+    }
+    if (residual_host) *residual_host = status ? 0.f : (float)h[27];
+    if (inlier_count_host) *inlier_count_host = status ? 0 : (int)h[28];
+    if (status) {  // TransformationConverter.cpp:219-225
+        set_last_error("Singular 6x6 linear system detected, tracking failed.");
+        return O3DB_ERR_SINGULAR;
+    }
+    return O3DB_OK;
+}
+
+void o3db_pose_to_symmetric_transformation(const double pose[6], const double source_mean[3], const double target_mean[3],
+                                           double transformation[16]) {
+    pose_to_symmetric_T(pose, source_mean, target_mean, transformation);
+}
+
+int o3db_compute_transformation_symmetric(const float* source_dev, const float* target_dev, const float* source_normals_dev,
+                                          const float* target_normals_dev, const int64_t* correspondences_dev, int64_t n,
+                                          int64_t m, const o3db_robust_kernel* kernel, double transformation_host[16],
+                                          int* inlier_count_host, void* stream) {
+    O3DB_REQUIRE(n > 0 && m > 0 && source_dev && target_dev && source_normals_dev && target_normals_dev &&
+                         correspondences_dev && transformation_host,
+                 "o3db_compute_transformation_symmetric: bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    double h[kSumStride], p[3];
+    {   // the means of the matched pairs, and the correspondence check
+        PoseScratch s;
+        if (int rc = pose_scratch_alloc(&s, n, st)) return rc;
+        symmetric_means_kernel<<<s.blocks, kThreads, 0, st>>>(source_dev, target_dev, correspondences_dev, n, m, s.partials,
+                                                              s.ticket, s.sums);
+        O3DB_LAUNCH_CHECK();
+        float pf[3];
+        O3DB_CUDA_CHECK(cudaMemcpyAsync(h, s.sums, sizeof(h), cudaMemcpyDeviceToHost, st));
+        O3DB_CUDA_CHECK(cudaMemcpyAsync(pf, target_dev, sizeof(pf), cudaMemcpyDeviceToHost, st));
+        O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
+        for (int k = 0; k < 3; ++k) p[k] = (double)pf[k];
+    }
+    if (h[29] > 0) {
+        set_last_error(kSymCorrMessage, (long long)m);
+        return O3DB_ERR_INVALID;
+    }
+    if (inlier_count_host) *inlier_count_host = (int)h[28];
+    if (h[28] == 0) {   // kernel/Registration.cpp:91-93
+        for (int i = 0; i < 16; ++i) transformation_host[i] = (i % 5 == 0) ? 1.0 : 0.0;
+        return O3DB_OK;
+    }
+    // the means in the cloud's dtype, as the reference's Tensor::Mean gives them to the kernel and the conversion
+    Vec3f ms, mt;
+    double ms64[3], mt64[3];
+    for (int k = 0; k < 3; ++k) {
+        ms.v[k] = (float)(p[k] + h[k] / h[28]);
+        mt.v[k] = (float)(p[k] + h[3 + k] / h[28]);
+        ms64[k] = ms.v[k];
+        mt64[k] = mt.v[k];
+    }
+    DevPtr<double> pose_dev;
+    if (int rc = dev_alloc(pose_dev, 6, st)) return rc;
+    int status = 0;
+    int rc = symmetric_pose_sums(source_dev, target_dev, source_normals_dev, target_normals_dev, correspondences_dev, n, m,
+                                 ms, mt, kernel, pose_dev.get(), h, &status, st);
+    if (rc) return rc;
+    if (status) {
+        set_last_error("Singular 6x6 linear system detected, tracking failed.");
+        return O3DB_ERR_SINGULAR;
+    }
+    double pose[6];
+    O3DB_CUDA_CHECK(cudaMemcpyAsync(pose, pose_dev.get(), sizeof(pose), cudaMemcpyDeviceToHost, st));
+    O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
+    pose_to_symmetric_T(pose, ms64, mt64, transformation_host);
+    return O3DB_OK;
+}
+
 int o3db_compute_information_matrix(const float* target_dev, const int64_t* correspondences_dev, int64_t n,
                                     double information_host[36], int64_t* num_correspondences_host, void* stream) {
     O3DB_REQUIRE(target_dev && correspondences_dev && information_host && n > 0, "o3db_compute_information_matrix: bad arguments");
@@ -1764,8 +2150,10 @@ void o3db_icp_destroy(o3db_icp* c) {
 }  // extern "C"
 
 namespace o3db {
-struct EstimatorInputs {   // all device pointers; null source_colors and no point_to_point = plain point-to-plane
+struct EstimatorInputs {   // all device pointers; null source_colors and source_normals and no point_to_point = plain
+                           // point-to-plane
     bool point_to_point = false;   // no target normals wanted
+    const float* source_normals = nullptr;   // symmetric
     const float* source_colors = nullptr;
     const float* target_colors = nullptr;
     const float* target_color_gradients = nullptr;
@@ -1795,6 +2183,8 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     c->n = n;
     c->comm = comm;
     c->point = col.point_to_point;
+    c->symmetric = col.source_normals != nullptr;
+    c->src_normals_user = col.source_normals;
     c->l2loss = c->point || options->kernel.method == O3DB_ROBUST_L2;
     c->colored = col.source_colors != nullptr;
     c->src_colors_user = col.source_colors;
@@ -1820,12 +2210,20 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     c->src_keys = ncell;
     // padded to whole 256-entry chunks: the staged kernel copies 32-entry chunks with TMA bulk copies
     c->n_pad = ceil_div(n, 256) * 256;
-    if ((rc = dev_alloc(c->src_blk, SrcBlocked::bytes(c->n_pad), st))) return rc;
+    if ((rc = dev_alloc(c->src_blk, c->symmetric ? SrcBlockedSym::bytes(c->n_pad) : SrcBlocked::bytes(c->n_pad), st)))
+        return rc;
     if ((rc = dev_alloc(c->src_idx, (size_t)c->n_pad, st))) return rc;
     // (no initial contents: IcpState::sums_cached starts at 0, so the first iteration writes every line)
     if ((rc = dev_alloc(c->chunk_sums, (size_t)c->n_pad, st))) return rc;
-    src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlocked{c->src_blk.get()}, n,
-                                                                                       c->n_pad, true);
+    if (c->symmetric) {
+        if ((rc = dev_alloc(c->chunk_sums2, (size_t)(c->n_pad / 32) * kSymLine2, st))) return rc;
+        if ((rc = dev_alloc(c->partials2, (size_t)c->grid_blocks * kSymLine2, st))) return rc;
+        src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlockedSym{c->src_blk.get()},
+                                                                                           n, c->n_pad, true);
+    } else {
+        src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlocked{c->src_blk.get()}, n,
+                                                                                           c->n_pad, true);
+    }
     O3DB_LAUNCH_CHECK();
     const size_t iter_sums = (size_t)std::max(1, options->max_iteration) * 2;
     if ((rc = dev_alloc(c->src_key, (size_t)n, st))) return rc;
@@ -1917,6 +2315,22 @@ int o3db_icp_create_point_to_point(const float* source_dev, int64_t n, const flo
     o3db::EstimatorInputs est;
     est.point_to_point = true;
     return icp_create_impl(source_dev, n, target_dev, nullptr, m, init_T, options, comm, est, stream, out);
+}
+
+int o3db_icp_create_symmetric(const float* source_dev, const float* source_normals_dev, int64_t n, const float* target_dev,
+                              const float* target_normals_dev, int64_t m, const double init_T[16],
+                              const o3db_icp_options* options, o3db_comm* comm, void* stream, o3db_icp** out) {
+    O3DB_REQUIRE(out != nullptr, "o3db_icp_create_symmetric: out is null");
+    *out = nullptr;
+    // TransformationEstimation.cpp:40-83 AssertValidSymmetricInputs
+    O3DB_REQUIRE(source_dev && target_dev && n > 0 && m > 0, "Source and/or Target pointcloud is empty.");
+    O3DB_REQUIRE(source_normals_dev != nullptr && target_normals_dev != nullptr,
+                 "SymmetricICP requires both source and target to have normals.");
+    // the in-kernel exchange and the NCCL path carry the 30 sums of one line; this estimator has a second line
+    O3DB_REQUIRE(comm == nullptr, "SymmetricICP does not run multi-GPU: pass no communicator.");
+    o3db::EstimatorInputs est;
+    est.source_normals = source_normals_dev;
+    return icp_create_impl(source_dev, n, target_dev, target_normals_dev, m, init_T, options, nullptr, est, stream, out);
 }
 
 int o3db_icp_reset(o3db_icp* c, void* stream) {
@@ -2013,6 +2427,20 @@ int o3db_icp_point_to_point(const float* source_dev, int64_t n, const float* tar
                             double* per_iteration_host, void* stream) {
     o3db_icp* c = nullptr;
     int rc = o3db_icp_create_point_to_point(source_dev, n, target_dev, m, init_T, options, nullptr, stream, &c);
+    if (rc) return rc;
+    rc = o3db_icp_iterate(c, options->max_iteration, stream);
+    if (rc == O3DB_OK) rc = o3db_icp_finish(c, result, correspondences_dev, per_iteration_host, stream);
+    cudaStreamSynchronize((cudaStream_t)stream);
+    o3db_icp_destroy(c);
+    return rc;
+}
+
+int o3db_icp_symmetric(const float* source_dev, const float* source_normals_dev, int64_t n, const float* target_dev,
+                       const float* target_normals_dev, int64_t m, const double init_T[16], const o3db_icp_options* options,
+                       o3db_icp_result* result, int64_t* correspondences_dev, double* per_iteration_host, void* stream) {
+    o3db_icp* c = nullptr;
+    int rc = o3db_icp_create_symmetric(source_dev, source_normals_dev, n, target_dev, target_normals_dev, m, init_T, options,
+                                       nullptr, stream, &c);
     if (rc) return rc;
     rc = o3db_icp_iterate(c, options->max_iteration, stream);
     if (rc == O3DB_OK) rc = o3db_icp_finish(c, result, correspondences_dev, per_iteration_host, stream);

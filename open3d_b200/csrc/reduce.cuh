@@ -4,7 +4,8 @@
 // stand-alone reductions; plus the f64 6x6 solve and pose -> transformation that the reference runs on the host
 // (kernel/TransformationConverter.cpp), and the on-device Gauss-Newton step built from them
 // (gauss_newton_step_warp, left_multiply_warp) that the fused ICP and odometry loops run on one warp; and the
-// point-to-point estimator's terms in the same slots with its f64 Kabsch step (kabsch_step_warp).
+// point-to-point estimator's terms in the same slots with its f64 Kabsch step (kabsch_step_warp), and the symmetric
+// estimator's raw terms with their recentring and half-angle step (symmetric_step_warp).
 #pragma once
 
 #include <utility>
@@ -42,12 +43,12 @@ __device__ __forceinline__ void flush_acc(float (&acc)[kNumSums], double (*s_war
 // unroller decides.  Written as nested loops over `half`, the sm_90a build kept v[] (and the callers' term arrays) in
 // local memory: 176 B of stack per thread, stored and reloaded through L1 / L2 for every 32-query chunk, which made the
 // ICP iteration 3.3x slower on an H100 (tests/test_local_memory.py guards against it).
-template <int HALF, int... K>
-__device__ __forceinline__ void warp_transpose_step(float (&v)[32], bool up, std::integer_sequence<int, K...>) {
+template <int HALF, int N, int... K>
+__device__ __forceinline__ void warp_transpose_step(float (&v)[N], bool up, std::integer_sequence<int, K...>) {
     ((v[K] = (up ? v[K + HALF] : v[K]) + __shfl_xor_sync(0xffffffffu, up ? v[K] : v[K + HALF], HALF)), ...);
 }
-template <int HALF>
-__device__ __forceinline__ void warp_transpose_steps(float (&v)[32], unsigned lane) {
+template <int HALF, int N>
+__device__ __forceinline__ void warp_transpose_steps(float (&v)[N], unsigned lane) {
     // step HALF: lane keeps v[k + HALF] (upper lane) or v[k] (lower lane) and adds what lane ^ HALF sends, k < HALF
     warp_transpose_step<HALF>(v, (lane & HALF) != 0, std::make_integer_sequence<int, HALF>{});
     if constexpr (HALF > 1) warp_transpose_steps<HALF / 2>(v, lane);
@@ -55,6 +56,16 @@ __device__ __forceinline__ void warp_transpose_steps(float (&v)[32], unsigned la
 __device__ __forceinline__ float warp_transpose_sum32(float (&v)[32]) {
     warp_transpose_steps<16>(v, threadIdx.x & 31u);
     return v[0];
+}
+// The same reduction at width 8 (the symmetric estimator's second line): three transposed steps leave lane l with
+// the sum of term l & 7 over its group of eight lanes, two butterfly steps add the four groups.  Every lane ends with
+// the same bits for its term (f32 addition commutes), so lanes 0-7 hold the line.
+__device__ __forceinline__ float warp_transpose_sum8(float (&v)[8]) {
+    warp_transpose_steps<4>(v, threadIdx.x & 31u);
+    float x = v[0];
+    x += __shfl_xor_sync(0xffffffffu, x, 8);
+    x += __shfl_xor_sync(0xffffffffu, x, 16);
+    return x;
 }
 
 // Block epilogue: per-warp slots -> block partial -> (last block) grand total in
@@ -454,6 +465,159 @@ __device__ __forceinline__ void kabsch_step_warp(const double* sums, const float
         U[15] = 1.0;
     }
     __syncwarp();
+}
+
+// -------------------------------------------------- symmetric step on one warp
+
+// Symmetric ICP's pose -> transformation (SymmetricICPImpl.h:19-43, Rusinkiewicz's equation 11) in f64: the pose's
+// rotation part g is the tangent of HALF the rotation angle, H = AngleAxis(atan|g|, g / |g|) (Rodrigues), R = H H and
+// t = mt + H (pose[3:6] cos(atan|g|)) - R ms, for the source and target means ms, mt the pose was solved about.
+// cos(atan x) = 1 / sqrt(1 + x^2) and sin(atan x) = x / sqrt(1 + x^2) replace the three trigonometric calls (whose f64
+// argument reduction would give the kernel a stack frame).
+__device__ __host__ inline void pose_to_symmetric_T(const double* pose, const double* ms, const double* mt, double* T) {
+    const double gn = sqrt(pose[0] * pose[0] + pose[1] * pose[1] + pose[2] * pose[2]);
+    const double c = 1.0 / sqrt(1.0 + gn * gn), s = gn * c, ic = 1.0 - c;
+    double H[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+    if (gn > 0.0) {
+        const double kx = pose[0] / gn, ky = pose[1] / gn, kz = pose[2] / gn;
+        H[0] = c + kx * kx * ic;
+        H[1] = kx * ky * ic - kz * s;
+        H[2] = kx * kz * ic + ky * s;
+        H[3] = ky * kx * ic + kz * s;
+        H[4] = c + ky * ky * ic;
+        H[5] = ky * kz * ic - kx * s;
+        H[6] = kz * kx * ic - ky * s;
+        H[7] = kz * ky * ic + kx * s;
+        H[8] = c + kz * kz * ic;
+    }
+    for (int i = 0; i < 3; ++i) {
+        double t = mt[i];
+        for (int k = 0; k < 3; ++k) {
+            double r = 0;
+            for (int j = 0; j < 3; ++j) r += H[3 * i + j] * H[3 * j + k];
+            T[4 * i + k] = r;
+            t += H[3 * i + k] * (pose[3 + k] * c);
+        }
+        T[4 * i + 3] = t;
+    }
+    for (int i = 0; i < 3; ++i)
+        for (int k = 0; k < 3; ++k) T[4 * i + 3] -= T[4 * i + k] * ms[k];
+    T[12] = T[13] = T[14] = 0.0;
+    T[15] = 1.0;
+}
+
+// Symmetric slot layout.  The 32-wide line holds, about a fixed pivot (s, t pivot-relative in f32), the raw system of
+// g = [u x n ; n] with u = s + t, n = n_t + sign(n_s . n_t) n_s and r = (s - t) . n: [0, 21) sum w g g^T (lower
+// triangle), [21, 27) sum w g r, [27] sum r^2, [28] count, [29] sum d^2.  The 8-wide second line holds [0, 3) sum s
+// and [3, 6) sum t; [6, 8) stay zero.  Every term is independent of the means, so both lines are linear over chunks.
+static constexpr int kSymSourceSum = 0, kSymTargetSum = 3, kSymLine2 = 8;
+
+template <bool L2LOSS, typename RobustW>
+__device__ __forceinline__ void accumulate_symmetric(float (&acc)[32], float (&acc2)[kSymLine2], const float (&s)[3],
+                                                     const float (&t)[3], const float (&ns)[3], const float (&nt)[3],
+                                                     RobustW&& weight) {
+    const float dot = ns[0] * nt[0] + ns[1] * nt[1] + ns[2] * nt[2];
+    const float sg = dot < 0.f ? -1.f : 1.f;
+    const float n[3] = {nt[0] + sg * ns[0], nt[1] + sg * ns[1], nt[2] + sg * ns[2]};
+    const float u[3] = {s[0] + t[0], s[1] + t[1], s[2] + t[2]};
+    const float r = (s[0] - t[0]) * n[0] + (s[1] - t[1]) * n[1] + (s[2] - t[2]) * n[2];
+    const float g[6] = {u[1] * n[2] - u[2] * n[1], u[2] * n[0] - u[0] * n[2], u[0] * n[1] - u[1] * n[0], n[0], n[1], n[2]};
+    const float w = L2LOSS ? 1.0f : weight(r);
+    int q = 0;
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+        const float gw = g[j] * w;
+#pragma unroll
+        for (int k = 0; k <= j; ++k) acc[q++] += gw * g[k];
+        acc[21 + j] += gw * r;
+    }
+    acc[27] += r * r;
+    acc[28] += 1.0f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        acc2[kSymSourceSum + k] += s[k];
+        acc2[kSymTargetSum + k] += t[k];
+    }
+}
+
+// The reference's centred system from the raw one, in f64, by ONE warp (lane q writes slot q < 29).  With ms, mt the
+// pivot-relative means, c = ms + mt, e = ms - mt and M = [[I, -[c]x], [0, I]] ([c]x n = c x n), the reference's Jacobian
+// is J = M g and its centred residual r_c = r - e . n, so J^T w J = M A M^T and J^T w r_c = M (b - A[:, 3:6] e).  Row j
+// of M has its diagonal 1 and, for j < 3, the three entries of -[c]x in columns 3-5.
+__device__ __forceinline__ double sym_A(const double* sums, int j, int k) {
+    const int hi = j > k ? j : k, lo = j > k ? k : j;
+    return sums[(hi * (hi + 1)) / 2 + lo];
+}
+__device__ __forceinline__ double sym_M(const double* c, int j, int l) {   // j < 3, l in 3..5: (-[c]x)[j][l - 3]
+    const int a = l - 3;
+    if (a == j) return 0.0;
+    const int o = 3 - j - a;   // the third axis (selected, not indexed: c stays in registers)
+    const double co = o == 0 ? c[0] : (o == 1 ? c[1] : c[2]);
+    return ((a - j + 3) % 3 == 1) ? co : -co;
+}
+__device__ __forceinline__ void symmetric_centre_warp(const double* sums, const double* ms, const double* mt, double* out) {
+    const int lane = threadIdx.x & 31;
+    const double c[3] = {ms[0] + mt[0], ms[1] + mt[1], ms[2] + mt[2]};
+    const double e[3] = {ms[0] - mt[0], ms[1] - mt[1], ms[2] - mt[2]};
+    if (lane < 21) {
+        int j = 0;
+        while ((j + 1) * (j + 2) / 2 <= lane) ++j;
+        const int k = lane - j * (j + 1) / 2;
+        double v = 0;
+        for (int li = 0; li < 4; ++li) {
+            if (li > 0 && j >= 3) break;
+            const int l = li == 0 ? j : 2 + li;
+            const double mjl = li == 0 ? 1.0 : sym_M(c, j, l);
+            for (int mi = 0; mi < 4; ++mi) {
+                if (mi > 0 && k >= 3) break;
+                const int m = mi == 0 ? k : 2 + mi;
+                const double mkm = mi == 0 ? 1.0 : sym_M(c, k, m);
+                v += mjl * sym_A(sums, l, m) * mkm;
+            }
+        }
+        out[lane] = v;
+    } else if (lane < 27) {
+        const int j = lane - 21;
+        double v = 0;
+        for (int li = 0; li < 4; ++li) {
+            if (li > 0 && j >= 3) break;
+            const int l = li == 0 ? j : 2 + li;
+            const double mjl = li == 0 ? 1.0 : sym_M(c, j, l);
+            const double be = sums[21 + l] - (sym_A(sums, l, 3) * e[0] + sym_A(sums, l, 4) * e[1] + sym_A(sums, l, 5) * e[2]);
+            v += mjl * be;
+        }
+        out[lane] = v;
+    } else if (lane < 29) {
+        out[lane] = sums[lane];
+    }
+}
+
+// The on-device part of one symmetric step, with gauss_newton_step_warp's calling convention (ONE warp, U left in
+// scratch[16, 32)); `scratch` needs 96 doubles: the centred system goes to [64, 93).  From the f64 totals of both
+// lines (sums[28] > 0): the means, the centred system, solve6x6_warp, and pose_to_symmetric_T about the world means.
+// Returns false on every lane for a singular system, and then leaves U unwritten.
+__device__ __forceinline__ bool symmetric_step_warp(const double* sums, const double* sums2, const float* pivot,
+                                                    double* scratch) {
+    const int lane = threadIdx.x & 31;
+    double* ms = scratch + 8;    // world means (read back by lane 0 after the solve)
+    double* mt = scratch + 11;
+    const double inv_n = 1.0 / sums[kCountSlot];
+    double rs[3], rt[3];
+    for (int k = 0; k < 3; ++k) {
+        rs[k] = sums2[kSymSourceSum + k] * inv_n;
+        rt[k] = sums2[kSymTargetSum + k] * inv_n;
+    }
+    if (lane == 0)
+        for (int k = 0; k < 3; ++k) {
+            ms[k] = rs[k] + (double)pivot[k];
+            mt[k] = rt[k] + (double)pivot[k];
+        }
+    symmetric_centre_warp(sums, rs, rt, scratch + 64);
+    __syncwarp();
+    if (!solve6x6_warp(scratch + 64, scratch + 16, scratch)) return false;
+    if (lane == 0) pose_to_symmetric_T(scratch, ms, mt, scratch + 16);
+    __syncwarp();
+    return true;
 }
 
 // T <- U T for 4 x 4 row-major matrices, by lanes 0-15 of a warp (all sixteen must call it): lane l writes T[l].

@@ -1,4 +1,4 @@
-"""Mirror of ``open3d.t.pipelines.registration`` for the point-to-point, point-to-plane and coloured ICP paths
+"""Mirror of ``open3d.t.pipelines.registration`` for the point-to-point, point-to-plane, symmetric and coloured ICP paths
 (cpp/pybind/t/pipelines/registration/registration.cpp:96-140, 469-530;
 cpp/open3d/t/pipelines/registration/{Registration,TransformationEstimation}.cpp).
 
@@ -252,6 +252,88 @@ class TransformationEstimationForColoredICP(TransformationEstimation):
         return T
 
 
+class TransformationEstimationSymmetric(TransformationEstimation):
+    """TransformationEstimation.h:214-270 / TransformationEstimation.cpp:229-292: Rusinkiewicz's symmetric objective,
+    residual (p - q) . (n_p +- n_q).  Both clouds need normals."""
+
+    def __init__(self, kernel: RobustKernel | None = None):
+        self.kernel = kernel if kernel is not None else RobustKernel()
+
+    @staticmethod
+    def _check(source, target):
+        """AssertValidSymmetricInputs (TransformationEstimation.cpp:40-83)."""
+        if not target.has_point_positions() or not source.has_point_positions():
+            raise RuntimeError("Source and/or Target pointcloud is empty.")
+        if "normals" not in source.point or "normals" not in target.point:
+            raise RuntimeError("SymmetricICP requires both source and target to have normals.")
+        for name, cloud in (("Source", source), ("Target", target)):
+            p, n = cloud.point["positions"], cloud.point["normals"]
+            if tuple(n.shape) != tuple(p.shape):
+                raise RuntimeError(f"{name} normals shape {list(n.shape)} must match {name.lower()} positions shape "
+                                   f"{list(p.shape)} for SymmetricICP.")
+
+    def _inputs(self, source, target, correspondences):
+        self._check(source, target)
+        s, t = source.point["positions"], target.point["positions"]
+        ns, nt = source.point["normals"], target.point["normals"]
+        return s, t, ns, nt, _corr_arg(correspondences, s.shape[0])
+
+    def compute_rmse(self, source, target, correspondences):
+        """TransformationEstimation.cpp:229-274: sqrt(mean(((s - t) . (sign n_s + n_t))^2)) over the valid pairs, 0 with
+        none (torch ops on the device, tensor ops upstream)."""
+        s, t, ns, nt, corr = self._inputs(source, target, correspondences)
+        if bool(((corr < -1) | (corr >= t.shape[0])).any()):
+            raise RuntimeError(f"SymmetricICP correspondences must be -1 or a target point index in [0, {t.shape[0]}), "
+                               "but an out-of-range value was found.")
+        valid = corr != -1
+        idx = corr[valid]
+        if idx.shape[0] == 0:
+            return 0.0
+        vs, vt, vns, vnt = s[valid], t[idx], ns[valid], nt[idx]
+        dot = (vns * vnt).sum(1, keepdim=True)
+        direction = torch.where(dot < 0, -1.0, 1.0).to(dot.dtype)
+        r = ((vs - vt) * (vns * direction + vnt)).sum(1)
+        return float(torch.sqrt((r * r).mean().to(torch.float64)))
+
+    def compute_pose(self, source, target, correspondences, source_mean, target_mean):
+        """kernel::ComputePoseSymmetric (RegistrationCPU.cpp:124-218) about the given means, through the C ABI seam
+        o3db_compute_pose_symmetric: pose [6] f64 on the device, residual (sum of squared objective residuals),
+        inlier_count and the 29 sums."""
+        s, t, ns, nt, corr = self._inputs(source, target, correspondences)
+        ms = (C.c_float * 3)(*[float(v) for v in np.asarray(source_mean, np.float32).reshape(3)])
+        mt = (C.c_float * 3)(*[float(v) for v in np.asarray(target_mean, np.float32).reshape(3)])
+        pose = torch.zeros(6, dtype=torch.float64, device=s.device)
+        sums = torch.zeros(29, dtype=torch.float64, device=s.device)
+        residual, count = C.c_float(0), C.c_int(0)
+        k = self.kernel._c()
+        check(lib.o3db_compute_pose_symmetric(s.data_ptr(), t.data_ptr(), ns.data_ptr(), nt.data_ptr(), corr.data_ptr(),
+                                              s.shape[0], t.shape[0], ms, mt, C.byref(k), sums.data_ptr(),
+                                              pose.data_ptr(), C.byref(residual), C.byref(count), current_stream_ptr()))
+        return pose, float(residual.value), int(count.value), sums
+
+    def compute_transformation(self, source, target, correspondences, current_transform=None, iteration=0):
+        """TransformationEstimation.cpp:276-292 (kernel::ComputeTransformationSymmetric) -> 4x4 Float64 on CPU; the
+        identity when no correspondence is valid."""
+        s, t, ns, nt, corr = self._inputs(source, target, correspondences)
+        T = np.zeros((4, 4), np.float64)
+        k = self.kernel._c()
+        check(lib.o3db_compute_transformation_symmetric(s.data_ptr(), t.data_ptr(), ns.data_ptr(), nt.data_ptr(),
+                                                        corr.data_ptr(), s.shape[0], t.shape[0], C.byref(k), dptr(T),
+                                                        None, current_stream_ptr()))
+        return T
+
+
+def pose_to_symmetric_transformation(pose, source_mean, target_mean):
+    """kernel::PoseToSymmetricTransformation (TransformationConverter.cpp:106-133, SymmetricICPImpl.h:19-43) on the
+    host in f64 -> 4x4."""
+    p = np.ascontiguousarray(np.asarray(pose, np.float64).reshape(6))
+    ms = np.ascontiguousarray(np.asarray(source_mean, np.float64).reshape(3))
+    mt = np.ascontiguousarray(np.asarray(target_mean, np.float64).reshape(3))
+    T = np.zeros((4, 4), np.float64)
+    lib.o3db_pose_to_symmetric_transformation(dptr(p), dptr(ms), dptr(mt), dptr(T))
+    return T
+
+
 def _options(max_correspondence_distance, criteria, kernel):
     o = IcpOptions()
     o.max_correspondence_distance = float(max_correspondence_distance)
@@ -267,9 +349,10 @@ def _assert_inputs(source, target, estimation_method, max_correspondence_distanc
     # Registration.cpp:119-219 AssertInputMultiScaleICP
     colored = isinstance(estimation_method, TransformationEstimationForColoredICP)
     if not colored and not isinstance(estimation_method, (TransformationEstimationPointToPoint,
-                                                          TransformationEstimationPointToPlane)):
-        raise RuntimeError("open3d_b200 implements TransformationEstimationPointToPoint, ...PointToPlane and "
-                           "...ForColoredICP; other estimators are outside this build's scope (SURVEY.md §8f).")
+                                                          TransformationEstimationPointToPlane,
+                                                          TransformationEstimationSymmetric)):
+        raise RuntimeError("open3d_b200 implements TransformationEstimationPointToPoint, ...Symmetric, ...PointToPlane "
+                           "and ...ForColoredICP; other estimators are outside this build's scope (SURVEY.md §8f).")
     if not target.has_point_positions() or not source.has_point_positions():
         raise RuntimeError("Source and/or Target pointcloud is empty.")
     if colored:
@@ -282,6 +365,8 @@ def _assert_inputs(source, target, estimation_method, max_correspondence_distanc
     elif isinstance(estimation_method, TransformationEstimationPointToPlane) and not target.has_point_normals():
         raise RuntimeError("TransformationEstimationPointToPlane require pre-computed normal vectors for target "
                            "PointCloud.")
+    elif isinstance(estimation_method, TransformationEstimationSymmetric):
+        TransformationEstimationSymmetric._check(source, target)
     if max_correspondence_distance <= 0.0:
         raise RuntimeError(" Max correspondence distance must be greater than 0, but got "
                            f"{max_correspondence_distance} in scale: {scale_idx}.")
@@ -319,6 +404,11 @@ def _run_single_scale(source, target, max_dist, init, estimation, criteria, call
             check(lib.o3db_icp_create_point_to_point(s.data_ptr(), s.shape[0], t.data_ptr(), t.shape[0], dptr(T0),
                                                      C.byref(opt), comm.handle if comm is not None else None, stream,
                                                      C.byref(handle)))
+        elif isinstance(estimation, TransformationEstimationSymmetric):
+            estimation._check(source, target)
+            ns, nt = source.point["normals"], target.point["normals"]
+            check(lib.o3db_icp_create_symmetric(s.data_ptr(), ns.data_ptr(), s.shape[0], t.data_ptr(), nt.data_ptr(),
+                                                t.shape[0], dptr(T0), C.byref(opt), None, stream, C.byref(handle)))
         else:
             n = target.point["normals"]
             check(lib.o3db_icp_create(s.data_ptr(), s.shape[0], t.data_ptr(), n.data_ptr(), t.shape[0], dptr(T0),
@@ -386,6 +476,16 @@ def icp(source, target, max_correspondence_distance, init_source_to_target=None,
                            callback_after_iteration, comm)
 
 
+def registration_symmetric_icp(source, target, max_correspondence_distance, init_source_to_target=None,
+                               estimation_method=None, criteria=None):
+    """registration_symmetric_icp (pybind/t/pipelines/registration/registration.cpp): ICP with
+    TransformationEstimationSymmetric() unless another symmetric estimator (e.g. with a robust kernel) is given."""
+    if estimation_method is None:
+        estimation_method = TransformationEstimationSymmetric()
+    return icp(source, target, max_correspondence_distance, init_source_to_target, estimation_method,
+               criteria or ICPConvergenceCriteria())
+
+
 def _shard(n, comm):
     from ....distributed import shard_range
     return shard_range(int(n), comm.rank, comm.world)
@@ -417,6 +517,9 @@ def multi_scale_icp(source, target, voxel_sizes, criteria_list, max_corresponden
     return the same transformation / fitness / rmse (correspondence_set covers the rank's own rows)."""
     if estimation_method is None:
         estimation_method = TransformationEstimationPointToPoint()   # Registration.h:140, 205
+    if comm is not None and isinstance(estimation_method, TransformationEstimationSymmetric):
+        # the multi-GPU exchange carries the 30 sums of one line; this estimator also sums both clouds' points
+        raise RuntimeError("TransformationEstimationSymmetric does not run multi-GPU: pass comm=None.")
     n_scales = len(criteria_list)
     if len(voxel_sizes) != n_scales or len(max_correspondence_distances) != n_scales:
         raise RuntimeError(" [MultiScaleICP]: Size of criterias, voxel_size, max_correspondence_distances vectors "
