@@ -87,6 +87,56 @@ int o3db_nns_hybrid_search(const o3db_nns* nns, const float* queries_dev /* [N,3
                            int32_t* indices_dev /* [N,max_knn] */, float* distances_dev /* [N,max_knn] */,
                            int32_t* counts_dev /* [N] */, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Exact k-nearest-neighbour search — replaces core::nns::NearestNeighborSearch::
+ * KnnIndex / KnnSearch (core/nns/NearestNeighborSearch.cpp:27-64, 93-113; on the
+ * GPU upstream runs core/nns/KnnSearchOps.cu, a brute-force GEMM, and on the CPU
+ * NanoFlannIndex::SearchKnn, NanoFlannIndex.cpp:62-118).
+ * The index owns a cell-sorted float4 copy of the points whose cell size is
+ * chosen from the data (DESIGN.md §4.17); `points_dev` may be freed after
+ * creation.  Creation synchronises `stream` once; a search does not.
+ * ---------------------------------------------------------------------- */
+typedef struct o3db_knn o3db_knn;
+
+enum { O3DB_INDEX_INT32 = 0, O3DB_INDEX_INT64 = 1 };
+
+/* Errors: an empty dataset, a non-finite coordinate. */
+int o3db_knn_create(const float* points_dev /* [M,3] */, int64_t num_points, void* stream, o3db_knn** out);
+void o3db_knn_destroy(o3db_knn* knn);
+
+/* The k' = min(knn, M) nearest dataset points of every query, knn in 1..32, ascending by
+ * (dist^2, index): exact ties resolve to the lower index.  dist^2 is
+ * fmaf(dz, dz, fmaf(dy, dy, dx * dx)) with d = point - query.  Indices are Int32 or
+ * Int64 (index_dtype), [N,k'] row-major like the distances; a query with a non-finite
+ * coordinate gets a row of -1 and 0.  num_queries == 0 is a no-op.  Either output may
+ * be NULL. */
+int o3db_knn_search(const o3db_knn* knn, const float* queries_dev /* [N,3] */, int64_t num_queries, int knn_k,
+                    int index_dtype, void* indices_dev /* [N,k'] */, float* distances_dev /* [N,k'] */,
+                    void* stream);
+
+/* The index's cell size, fine-cell count and coarse-block count (diagnostics). */
+int o3db_knn_index_stats(const o3db_knn* knn, double* cell_size, int64_t* num_cells, int64_t* num_blocks);
+
+/* PointCloud::RemoveStatisticalOutliers (t/geometry/PointCloud.cpp:678-714): mask[i] =
+ * avg[i] <= (float)(cloud_mean + std_ratio * std), avg[i] = the mean distance to the
+ * k' = min(nb_neighbors, n) nearest points (the point itself included).  The two
+ * cloud-wide sums are taken in f64 in a fixed order (upstream: f32, in an order that
+ * depends on its reduction), so repeated calls are bit-identical; DESIGN.md §4.17 gives
+ * every operation.  nb_neighbors in 1..32.  avg_dev may be NULL.  n == 0 is a no-op;
+ * n == 1 keeps nothing (the standard deviation is NaN), as upstream.  Synchronises. */
+int o3db_remove_statistical_outliers(const float* positions_dev, int64_t n, int nb_neighbors, double std_ratio,
+                                     uint8_t* mask_dev /* [n] */, float* avg_dev /* [n] or NULL */, void* stream);
+
+/* PointCloud::ComputeMetrics (t/geometry/PointCloud.cpp:1805-1835, kernel/Metrics.cpp):
+ * two 1-NN searches on the device, then the values in the order of `metrics`, FScore
+ * giving one value per radius, into values_host (num_values at least that many).  Counts
+ * of distances below a radius are exact integers (upstream counts in f32, exact only up
+ * to 2^24 points).  Synchronises. */
+enum { O3DB_METRIC_CHAMFER = 0, O3DB_METRIC_HAUSDORFF = 1, O3DB_METRIC_FSCORE = 2 };
+int o3db_compute_metrics(const float* points1_dev, int64_t n1, const float* points2_dev, int64_t n2,
+                         const int* metrics_host, int num_metrics, const float* fscore_radius_host, int num_radius,
+                         float* values_host, int64_t num_values, void* stream);
+
 /* Reference-layout CSR spatial hash (parity / interop only): exactly the tables
  * BuildSpatialHashTableCUDA produces — cell = floor(p/(2r)), bucket =
  * SpatialHash(cell) % hash_table_size (core/nns/NeighborSearchCommon.h:31-52),

@@ -16,6 +16,8 @@ ERR_INVALID, ERR_CUDA, ERR_SINGULAR, ERR_CAPACITY, ERR_NO_BLOCKS, ERR_COMM, ERR_
 DEPTH_U16, DEPTH_F32 = 0, 1
 COLOR_NONE, COLOR_U8, COLOR_F32 = 0, 1, 2
 UNIQUE_ID_BYTES = 128
+INDEX_INT32, INDEX_INT64 = 0, 1
+METRIC_CHAMFER, METRIC_HAUSDORFF, METRIC_FSCORE = 0, 1, 2
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(
@@ -70,6 +72,12 @@ _SIGS = {
     "o3db_nns_create": (_i, [_vp, _i64, _dbl, _vp, C.POINTER(_vp)]),
     "o3db_nns_destroy": (None, [_vp]),
     "o3db_nns_hybrid_search": (_i, [_vp, _vp, _i64, _dbl, _i, _vp, _vp, _vp, _vp]),
+    "o3db_knn_create": (_i, [_vp, _i64, _vp, C.POINTER(_vp)]),
+    "o3db_knn_destroy": (None, [_vp]),
+    "o3db_knn_search": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp, _vp]),
+    "o3db_knn_index_stats": (_i, [_vp, _dp, C.POINTER(_i64), C.POINTER(_i64)]),
+    "o3db_remove_statistical_outliers": (_i, [_vp, _i64, _i, _dbl, _vp, _vp, _vp]),
+    "o3db_compute_metrics": (_i, [_vp, _i64, _vp, _i64, _vp, _i, _vp, _i, _vp, _i64, _vp]),
     "o3db_compute_pose_point_to_plane": (_i, [_vp, _vp, _vp, _vp, _i64, C.POINTER(RobustKernel), _vp, _vp,
                                               C.POINTER(_f), C.POINTER(_i), _vp]),
     "o3db_compute_pose_colored_icp": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(RobustKernel), _dbl,

@@ -50,3 +50,6 @@ def as_host_f64_4x4(T, name="transformation") -> np.ndarray:
     if T.shape != (4, 4):
         raise RuntimeError(f"{name}: expected shape [4, 4], got {T.shape}")
     return T
+
+
+from . import nns  # noqa: E402,F401  (uses the helpers above)

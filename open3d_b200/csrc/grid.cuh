@@ -32,6 +32,34 @@ struct Grid {
     int ax[3];
 };
 
+}  // namespace o3db
+
+// A cell-sorted copy of a point set: the hybrid search's index (o3db_nns), the fused ICP target and, inside
+// o3db_knn, the k-nearest-neighbour index.
+struct o3db_nns {
+    cudaStream_t stream = 0;   // creation stream (buffers are freed on it)
+    o3db::Grid g{};
+    double radius = 0;
+    int64_t m = 0;
+    int64_t ncell = 0;
+    o3db::DevPtr<float4> pts4;
+    o3db::DevPtr<float4> nrm4;
+    o3db::DevPtr<unsigned> cell_start;
+};
+
+namespace o3db {
+
+// The index build (icp.cu, DESIGN.md §4.2), in the pieces its two callers share:
+// bbox_launch    bbox_kernel into d_bbox[6] (ordered-uint min xyz, max xyz) on st, without synchronising;
+// bbox_decode    the read-back box; an error for non-finite coordinates;
+// grid_from_bbox the grid of cell size c (grown by 1.25x until it fits the cell caps); thin_cells: grid-x cells
+//                kThinFactor coarser, and the thin axis merged into one cell for sparse columns (the hybrid search)
+// grid_sort      s->g / s->ncell set: the counting sort into s->pts4 / s->nrm4 / s->cell_start.
+int bbox_launch(const float* pts, int64_t m, unsigned* d_bbox, cudaStream_t st);
+int bbox_decode(const unsigned h_bbox[6], float mn[3], float mx[3]);
+void grid_from_bbox(const float mn[3], const float mx[3], double c, bool thin_cells, int64_t m, Grid* g, int64_t* ncell);
+int grid_sort(o3db_nns* s, const float* pts, const float* nrm, int64_t m, cudaStream_t st);
+
 __device__ __forceinline__ float pick_axis(int a, float x, float y, float z) { return a == 0 ? x : (a == 1 ? y : z); }
 // real (x,y,z) -> grid-ordered (gx,gy,gz)
 __device__ __forceinline__ void to_grid(const Grid& g, float x, float y, float z, float& gx, float& gy, float& gz) {
@@ -337,7 +365,7 @@ __device__ __forceinline__ unsigned nn_search_seeded_fast(const Grid& g, const f
 //   then:      the full-radius box (or the seed-bounded one) as one flat 5-slab scan;
 //   otherwise: the pruned row-by-row search.
 // Returns the winner's sorted position or kNoPoint.
-__device__ __noinline__ unsigned nn_search_slow(const Grid* gp, const float4* __restrict__ pts,
+static __device__ __noinline__ unsigned nn_search_slow(const Grid* gp, const float4* __restrict__ pts,
                                                 const unsigned* __restrict__ cs, float qx, float qy, float qz,
                                                 float r1, float r1_accept2, float rr, float thr, int seed_j) {
     const Grid& g = *gp;

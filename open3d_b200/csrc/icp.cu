@@ -340,25 +340,13 @@ __global__ void ref_scatter_kernel(const float* __restrict__ pts, int64_t n, flo
 
 using namespace o3db;
 
-struct o3db_nns {
-    cudaStream_t stream = 0;   // creation stream (buffers are freed on it)
-    Grid g{};
-    double radius = 0;
-    int64_t m = 0;
-    int64_t ncell = 0;
-    DevPtr<float4> pts4;
-    DevPtr<float4> nrm4;
-    DevPtr<unsigned> cell_start;
-};
-
 namespace o3db {
 
 using NnsPtr = std::unique_ptr<o3db_nns, HandleDestroy<o3db_nns_destroy>>;
 
 static constexpr double kThinMergeMax = 8.0;   // merge the whole thin axis into ONE cell while a (y, z) column holds at most this many points on average
-static int grid_from_bbox(const float mn[3], const float mx[3], double radius, double cell_scale, int64_t m, Grid* g,
-                          int64_t* ncell) {
-    double c = radius * (cell_scale > 0 ? cell_scale : 1.0) * (1.0 + 1e-4);
+void grid_from_bbox(const float mn[3], const float mx[3], double c, bool thin_cells, int64_t m, Grid* g,
+                    int64_t* ncell) {
     if (!(c > 0) || !std::isfinite(c)) c = 1.0;
     double ext[3];
     double maxabs = 0;
@@ -380,8 +368,8 @@ static int grid_from_bbox(const float mn[3], const float mx[3], double radius, d
         // extent, the thin axis becomes a single cell (slab scans cross all of it anyway): the CSR table
         // shrinks by nx and a slab boundary is one multiply-free lookup.  Volumetric clouds keep thin cells.
         const double cols = (std::floor(ext[order[1]] / c) + 1) * (std::floor(ext[order[2]] / c) + 1);
-        cx = c * kThinFactor;
-        if ((double)m <= kThinMergeMax * cols) cx = std::max(cx, ext[order[0]] * (1.0 + 1e-3) + c);
+        cx = thin_cells ? c * kThinFactor : c;
+        if (thin_cells && (double)m <= kThinMergeMax * cols) cx = std::max(cx, ext[order[0]] * (1.0 + 1e-3) + c);
         for (int k = 0; k < 3; ++k) {
             n[k] = std::floor(ext[order[k]] / (k == 0 ? cx : c)) + 1;
             ok = ok && n[k] <= kMaxCellsPerAxis;
@@ -408,30 +396,18 @@ static int grid_from_bbox(const float mn[3], const float mx[3], double radius, d
         g->bmax[k] = mx[order[k]];
     }
     *ncell = (int64_t)g->nx * g->ny * g->nz;
+}
+
+int bbox_launch(const float* pts, int64_t m, unsigned* d_bbox, cudaStream_t st) {
+    const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
+    O3DB_CUDA_CHECK(cudaMemcpyAsync(d_bbox, init, sizeof(init), cudaMemcpyHostToDevice, st));
+    const int blocks = (int)std::min<int64_t>(ceil_div(m, kThreads), (int64_t)num_sms() * 8);
+    bbox_kernel<<<blocks, kThreads, 0, st>>>(pts, m, d_bbox);
+    O3DB_LAUNCH_CHECK();
     return O3DB_OK;
 }
 
-// Builds pts4 / nrm4 / cell_start for `pts` (device).  Synchronises `st` once
-// (the grid dimensions depend on the bounding box).
-static int nns_build(o3db_nns* s, const float* pts, const float* nrm, int64_t m, double radius,
-                     double cell_scale, cudaStream_t st) {
-    configure_memory_pool();
-    s->stream = st;
-    s->m = m;
-    s->radius = radius;
-    unsigned h_bbox[6];
-    {
-        DevPtr<unsigned> d_bbox;
-        if (int rc = dev_alloc(d_bbox, 6, st)) return rc;
-        const unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
-        O3DB_CUDA_CHECK(cudaMemcpyAsync(d_bbox.get(), init, sizeof(init), cudaMemcpyHostToDevice, st));
-        const int blocks = (int)std::min<int64_t>(ceil_div(m, kThreads), (int64_t)num_sms() * 8);
-        bbox_kernel<<<blocks, kThreads, 0, st>>>(pts, m, d_bbox.get());
-        O3DB_LAUNCH_CHECK();
-        O3DB_CUDA_CHECK(cudaMemcpyAsync(h_bbox, d_bbox.get(), sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
-        O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
-    }
-    float mn[3], mx[3];
+int bbox_decode(const unsigned h_bbox[6], float mn[3], float mx[3]) {
     for (int a = 0; a < 3; ++a) {
         mn[a] = ordered_to_float(h_bbox[a]);
         mx[a] = ordered_to_float(h_bbox[3 + a]);
@@ -440,8 +416,10 @@ static int nns_build(o3db_nns* s, const float* pts, const float* nrm, int64_t m,
             return O3DB_ERR_INVALID;
         }
     }
-    grid_from_bbox(mn, mx, radius, cell_scale, m, &s->g, &s->ncell);
+    return O3DB_OK;
+}
 
+int grid_sort(o3db_nns* s, const float* pts, const float* nrm, int64_t m, cudaStream_t st) {
     DevPtr<unsigned> key, rank, scratch;
     if (int rc = dev_alloc(s->cell_start, (size_t)(s->ncell + 1), st)) return rc;
     if (int rc = dev_alloc(s->pts4, (size_t)m, st)) return rc;
@@ -464,6 +442,28 @@ static int nns_build(o3db_nns* s, const float* pts, const float* nrm, int64_t m,
                                                    s->nrm4.get());
     O3DB_LAUNCH_CHECK();
     return O3DB_OK;
+}
+
+// Builds pts4 / nrm4 / cell_start for `pts` (device), cells of radius x cell_scale.  Synchronises `st` once
+// (the grid dimensions depend on the bounding box).
+static int nns_build(o3db_nns* s, const float* pts, const float* nrm, int64_t m, double radius,
+                     double cell_scale, cudaStream_t st) {
+    configure_memory_pool();
+    s->stream = st;
+    s->m = m;
+    s->radius = radius;
+    unsigned h_bbox[6];
+    {
+        DevPtr<unsigned> d_bbox;
+        if (int rc = dev_alloc(d_bbox, 6, st)) return rc;
+        if (int rc = bbox_launch(pts, m, d_bbox.get(), st)) return rc;
+        O3DB_CUDA_CHECK(cudaMemcpyAsync(h_bbox, d_bbox.get(), sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
+        O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
+    }
+    float mn[3], mx[3];
+    if (int rc = bbox_decode(h_bbox, mn, mx)) return rc;
+    grid_from_bbox(mn, mx, radius * (cell_scale > 0 ? cell_scale : 1.0) * (1.0 + 1e-4), true, m, &s->g, &s->ncell);
+    return grid_sort(s, pts, nrm, m, st);
 }
 
 // ------------------------------------------------------- stand-alone search

@@ -7,15 +7,33 @@
 from __future__ import annotations
 
 import ctypes as C
+import enum
 import weakref
 
 import numpy as np
 import torch
 
 from .. import _libshim as _s
-from ..._lib import (COLOR_F32, COLOR_NONE, COLOR_U8, DEPTH_F32, DEPTH_U16, ERR_CAPACITY, O3DBError, check, dptr, lib)
+from ..._lib import (COLOR_F32, COLOR_NONE, COLOR_U8, DEPTH_F32, DEPTH_U16, ERR_CAPACITY, METRIC_CHAMFER, METRIC_FSCORE,
+                     METRIC_HAUSDORFF, O3DBError, check, dptr, lib)
 from ._replay import FrameReplay
 from ...core import as_device_f32_points, as_host_f64_4x4, current_stream_ptr
+
+
+class Metric(enum.IntEnum):
+    """t::geometry::Metric (t/geometry/Geometry.h:98-102)."""
+    ChamferDistance = METRIC_CHAMFER
+    HausdorffDistance = METRIC_HAUSDORFF
+    FScore = METRIC_FSCORE
+
+
+class MetricParameters:
+    """t::geometry::MetricParameters (t/geometry/Geometry.h:104-113): the F-score radii, and the sample count that
+    only mesh metrics use."""
+
+    def __init__(self, fscore_radius=(0.01,), n_sampled_points=1000):
+        self.fscore_radius = [float(r) for r in fscore_radius]
+        self.n_sampled_points = int(n_sampled_points)
 
 
 class PointCloud:
@@ -244,6 +262,43 @@ class PointCloud:
                                float(depth_scale), float(depth_max), height, width, depth.data_ptr(),
                                None if color is None else color.data_ptr(), current_stream_ptr()))
         return depth, color
+
+    def remove_statistical_outliers(self, nb_neighbors, std_ratio):
+        """PointCloud::RemoveStatisticalOutliers (t/geometry/PointCloud.cpp:678-714) -> (PointCloud, mask): keeps the
+        points whose mean distance to their nb_neighbors (1..32) nearest points, itself included, is at most
+        mean + std_ratio * std over the cloud.  The mask is a torch.bool on the device; every attribute is selected by
+        it in the original order.  The cloud-wide sums are exact-order f64 (o3db_remove_statistical_outliers)."""
+        if nb_neighbors < 1 or std_ratio <= 0:
+            raise RuntimeError("Illegal input parameters, the number of neighbors and standard deviation ratio must "
+                               "be positive.")
+        p = self._positions_f32("RemoveStatisticalOutliers")
+        n = int(p.shape[0])
+        mask = torch.empty((n,), dtype=torch.bool, device=p.device)
+        if n == 0:
+            return PointCloud(), mask
+        check(lib.o3db_remove_statistical_outliers(p.data_ptr(), n, int(nb_neighbors), float(std_ratio),
+                                                   mask.data_ptr(), None, current_stream_ptr()))
+        out = PointCloud()
+        out.point = {k: v[mask] for k, v in self.point.items()}
+        return out, mask
+
+    def compute_metrics(self, pcd2, metrics, params=None):
+        """PointCloud::ComputeMetrics (t/geometry/PointCloud.cpp:1805-1835, kernel/Metrics.cpp) -> a CPU Float32
+        tensor with the values of `metrics` in order, Metric.FScore giving one value per params.fscore_radius.  Both
+        nearest-neighbour searches run on the device, where upstream copies the clouds to the CPU."""
+        params = MetricParameters() if params is None else params
+        if not self.has_point_positions() or not pcd2.has_point_positions():
+            raise RuntimeError("One or both input point clouds are empty!")
+        p1 = self._positions_f32("ComputeMetrics")
+        p2 = pcd2._positions_f32("ComputeMetrics")
+        ms = np.ascontiguousarray([int(Metric(m)) for m in metrics], np.int32)
+        radius = np.ascontiguousarray(params.fscore_radius, np.float32)
+        nval = sum(len(radius) if m == METRIC_FSCORE else 1 for m in ms)
+        out = np.zeros(max(nval, 1), np.float32)
+        check(lib.o3db_compute_metrics(p1.data_ptr(), int(p1.shape[0]), p2.data_ptr(), int(p2.shape[0]), ms.ctypes.data,
+                                       len(ms), radius.ctypes.data, len(radius), out.ctypes.data, nval,
+                                       current_stream_ptr()))
+        return torch.from_numpy(out[:nval].copy())
 
     def _positions_f32(self, who):
         p = self.point.get("positions")
