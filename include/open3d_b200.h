@@ -137,6 +137,41 @@ int o3db_compute_metrics(const float* points1_dev, int64_t n1, const float* poin
                          const int* metrics_host, int num_metrics, const float* fscore_radius_host, int num_radius,
                          float* values_host, int64_t num_values, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Point-cloud smoothing — t::geometry::PointCloud::SmoothLaplacian / SmoothTaubin /
+ * SmoothMLS / SmoothBilateral (t/geometry/PointCloud.cpp:1074-1198, kernel/
+ * PointCloudImpl.h:1341-1753), Float32.  The arithmetic is upstream's, in f32 in
+ * neighbour-list order; exp is evaluated in f64 and rounded to f32 (DESIGN.md §4.18).
+ * out_dev [n,3] must not alias positions_dev.  n == 0 is a no-op.
+ * ---------------------------------------------------------------------- */
+
+/* SmoothLaplacian / SmoothTaubin: `iterations` rounds of num_factors (1 or 2) passes,
+ * pass j of a round using factors_host[j] (Laplacian: {lambda}; Taubin: {lambda, mu}).
+ * Each pass moves every point by factor x (mean of its k' = min(n, max_nn + 1) nearest
+ * points other than itself - the point); k' <= 32.  The neighbourhoods are searched
+ * again before every pass, over the current positions, unless fixed_neighborhoods,
+ * when the first search serves every pass.  iterations == 0 or max_nn <= 0 copies the
+ * positions.  Each index build synchronises once. */
+int o3db_smooth_laplacian(const float* positions_dev, int64_t n, int64_t iterations, const double* factors_host,
+                          int num_factors, int max_nn, int fixed_neighborhoods, float* out_dev, void* stream);
+
+/* SmoothMLS: each point projected onto the plane of the Gaussian-weighted PCA of its
+ * neighbours (fewer than 3: unchanged).  radius > 0 and max_nn in 1..32: the hybrid
+ * search; radius <= 0: the min(n, max_nn) <= 32 nearest points with weight 1; radius
+ * <= 0 and max_nn <= 0 copies the positions; max_nn <= 0 with radius > 0 (upstream's
+ * fixed-radius search) is an error.  normals_dev [n,3] (in/out, or NULL): the fitted
+ * plane's normal, or the old normal normalised where no plane is fitted. */
+int o3db_smooth_mls(const float* positions_dev, int64_t n, double radius, int max_nn, float* out_dev,
+                    float* normals_dev, void* stream);
+
+/* SmoothBilateral: each point with more than one hybrid-search neighbour (radius > 0,
+ * max_nn in 1..32) becomes the mean of its neighbours weighted by
+ * exp(-d^2 / (2 sigma_s^2) - r^2 / (2 sigma_r^2)), r the offset along its normal.
+ * sigma_s, sigma_r > 0.  normals_dev is required (upstream estimates missing normals
+ * with its KNN-only EstimateNormals, which this build does not have). */
+int o3db_smooth_bilateral(const float* positions_dev, const float* normals_dev, int64_t n, double radius, int max_nn,
+                          double sigma_s, double sigma_r, float* out_dev, void* stream);
+
 /* Reference-layout CSR spatial hash (parity / interop only): exactly the tables
  * BuildSpatialHashTableCUDA produces — cell = floor(p/(2r)), bucket =
  * SpatialHash(cell) % hash_table_size (core/nns/NeighborSearchCommon.h:31-52),

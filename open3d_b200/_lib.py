@@ -78,6 +78,9 @@ _SIGS = {
     "o3db_knn_index_stats": (_i, [_vp, _dp, C.POINTER(_i64), C.POINTER(_i64)]),
     "o3db_remove_statistical_outliers": (_i, [_vp, _i64, _i, _dbl, _vp, _vp, _vp]),
     "o3db_compute_metrics": (_i, [_vp, _i64, _vp, _i64, _vp, _i, _vp, _i, _vp, _i64, _vp]),
+    "o3db_smooth_laplacian": (_i, [_vp, _i64, _i64, _dp, _i, _i, _i, _vp, _vp]),
+    "o3db_smooth_mls": (_i, [_vp, _i64, _dbl, _i, _vp, _vp, _vp]),
+    "o3db_smooth_bilateral": (_i, [_vp, _vp, _i64, _dbl, _i, _dbl, _dbl, _vp, _vp]),
     "o3db_compute_pose_point_to_plane": (_i, [_vp, _vp, _vp, _vp, _i64, C.POINTER(RobustKernel), _vp, _vp,
                                               C.POINTER(_f), C.POINTER(_i), _vp]),
     "o3db_compute_pose_colored_icp": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(RobustKernel), _dbl,

@@ -300,6 +300,69 @@ class PointCloud:
                                        current_stream_ptr()))
         return torch.from_numpy(out[:nval].copy())
 
+    def smooth_laplacian(self, iterations=10, lambda_=0.5, max_nn=20, use_fixed_neighborhoods=False):
+        """PointCloud::SmoothLaplacian (t/geometry/PointCloud.cpp:1106-1131) -> a new PointCloud: `iterations` passes
+        of x_i <- x_i + lambda_ * (mean of its neighbours - x_i) over the max_nn + 1 nearest points (itself excluded),
+        searched again before every pass unless use_fixed_neighborhoods.  Every other attribute is cloned."""
+        return self._smooth_knn("SmoothLaplacian", iterations, (lambda_,), max_nn, use_fixed_neighborhoods)
+
+    def smooth_taubin(self, iterations=10, lambda_=0.5, mu=-0.53, max_nn=20, use_fixed_neighborhoods=False):
+        """PointCloud::SmoothTaubin (t/geometry/PointCloud.cpp:1133-1158) -> a new PointCloud: each iteration is a
+        Laplacian pass with lambda_ and then one with mu (see smooth_laplacian)."""
+        return self._smooth_knn("SmoothTaubin", iterations, (lambda_, mu), max_nn, use_fixed_neighborhoods)
+
+    def smooth_mls(self, radius=0.05, max_nn=30):
+        """PointCloud::SmoothMLS (t/geometry/PointCloud.cpp:1074-1104) -> a new PointCloud: each point projected onto
+        the plane of the Gaussian-weighted PCA of its hybrid-search neighbours (radius <= 0: its max_nn nearest points,
+        each of weight 1).  The cloud's normals, if it has them, become the planes' normals."""
+        p = self._positions_f32("SmoothMLS")
+        out = self.clone()
+        n = int(p.shape[0])
+        if n == 0:
+            return out
+        nrm = None
+        if self.has_point_normals():
+            nrm = out.point["normals"] = self._normals_f32(n).clone()
+        pos = out.point["positions"] = torch.empty_like(p)
+        check(lib.o3db_smooth_mls(p.data_ptr(), n, float(radius), int(max_nn), pos.data_ptr(),
+                                  None if nrm is None else nrm.data_ptr(), current_stream_ptr()))
+        return out
+
+    def smooth_bilateral(self, radius=0.05, max_nn=30, sigma_s=0.05, sigma_r=0.05):
+        """PointCloud::SmoothBilateral (t/geometry/PointCloud.cpp:1160-1198) -> a new PointCloud carrying the normals:
+        each point becomes the mean of its hybrid-search neighbours weighted by their distance (sigma_s) and their
+        offset along its normal (sigma_r).  The cloud must have normals (see estimate_normals)."""
+        p = self._positions_f32("SmoothBilateral")
+        n = int(p.shape[0])
+        if n == 0:
+            return self.clone()
+        if sigma_s <= 0 or sigma_r <= 0:
+            raise RuntimeError("Sigma values must be positive.")
+        if not self.has_point_normals():
+            raise RuntimeError("SmoothBilateral needs normals: upstream estimates missing ones with the KNN-only "
+                               "EstimateNormals(), which open3d_b200 does not build. Call estimate_normals(max_nn, "
+                               "radius) first.")
+        out = self.clone()
+        nrm = out.point["normals"] = self._normals_f32(n).clone()
+        pos = out.point["positions"] = torch.empty_like(p)
+        check(lib.o3db_smooth_bilateral(p.data_ptr(), nrm.data_ptr(), n, float(radius), int(max_nn), float(sigma_s),
+                                        float(sigma_r), pos.data_ptr(), current_stream_ptr()))
+        return out
+
+    def _smooth_knn(self, who, iterations, factors, max_nn, fixed):
+        p = self._positions_f32(who)
+        if iterations < 0:
+            raise RuntimeError(f"{who}: iterations must be non-negative (upstream takes a size_t), got {iterations}")
+        out = self.clone()
+        n = int(p.shape[0])
+        if n == 0:
+            return out
+        f = np.ascontiguousarray(factors, np.float64)
+        pos = out.point["positions"] = torch.empty_like(p)
+        check(lib.o3db_smooth_laplacian(p.data_ptr(), n, int(iterations), dptr(f), len(f), int(max_nn), int(bool(fixed)),
+                                        pos.data_ptr(), current_stream_ptr()))
+        return out
+
     def _positions_f32(self, who):
         p = self.point.get("positions")
         if p is None:
