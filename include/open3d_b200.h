@@ -172,6 +172,26 @@ int o3db_smooth_mls(const float* positions_dev, int64_t n, double radius, int ma
 int o3db_smooth_bilateral(const float* positions_dev, const float* normals_dev, int64_t n, double radius, int max_nn,
                           double sigma_s, double sigma_r, float* out_dev, void* stream);
 
+/* ------------------------------------------------------------------------
+ * DBSCAN clustering — t::geometry::PointCloud::ClusterDBSCAN (t/geometry/PointCloud.cpp:
+ * 1634-1644), which runs geometry::PointCloud::ClusterDBSCAN (geometry/PointCloudCluster.cpp:
+ * 21-97) on the host; Float32.  labels_dev [n] receives upstream's labels exactly (DESIGN.md
+ * §4.19):
+ *   neighbours  j of i iff d2 < eps * eps, d2 = ((0 + dx dx) + dy dy) + dz dz in f64 on the
+ *               f32 coordinates, dx = x_i - x_j, no FMA (nanoflann's metric and radius test,
+ *               reached through KDTreeFlann::SearchRadius, geometry/KDTreeFlann.cpp:114-135);
+ *   core        at least min_points neighbours, the point itself included (:57);
+ *   clusters    the connected components of the core points, numbered 0, 1, ... in the
+ *               order of each component's smallest index (:50-94);
+ *   border      a non-core point with a core neighbour takes the smallest cluster id among
+ *               its core neighbours (:76); every other point is noise, -1.
+ * Errors, before any CUDA call: null pointers, n < 0 or n >= INT_MAX, eps <= 0 or not finite,
+ * min_points < 0; from the index build: a non-finite coordinate.  n == 0 is a no-op.
+ * Synchronises once (the index build's bounding box); the launches depend on the arguments
+ * only. */
+int o3db_cluster_dbscan(const float* positions_dev /* [n,3] */, int64_t n, double eps, int64_t min_points,
+                        int32_t* labels_dev /* [n] */, void* stream);
+
 /* Reference-layout CSR spatial hash (parity / interop only): exactly the tables
  * BuildSpatialHashTableCUDA produces — cell = floor(p/(2r)), bucket =
  * SpatialHash(cell) % hash_table_size (core/nns/NeighborSearchCommon.h:31-52),

@@ -349,6 +349,22 @@ class PointCloud:
                                         float(sigma_r), pos.data_ptr(), current_stream_ptr()))
         return out
 
+    def cluster_dbscan(self, eps, min_points, print_progress=False):
+        """PointCloud::ClusterDBSCAN (t/geometry/PointCloud.cpp:1634-1644, geometry/PointCloudCluster.cpp:21-97) -> a
+        torch.int32 tensor [n] on the cloud's device: the DBSCAN cluster of every point, -1 for noise.  Points closer
+        than eps are neighbours; a point with at least min_points neighbours, itself included, is a core point.  The
+        clusters are numbered in the order of their smallest point index, and a border point takes the lowest cluster
+        id among its core neighbours, so the labels are upstream's exactly.  print_progress is accepted and ignored."""
+        del print_progress
+        p = self._positions_f32("ClusterDBSCAN")
+        n = int(p.shape[0])
+        labels = torch.empty((n,), dtype=torch.int32, device=p.device)
+        if n == 0:
+            return labels
+        check(lib.o3db_cluster_dbscan(p.data_ptr(), n, float(eps), int(min_points), labels.data_ptr(),
+                                      current_stream_ptr()))
+        return labels
+
     def _smooth_knn(self, who, iterations, factors, max_nn, fixed):
         p = self._positions_f32(who)
         if iterations < 0:
