@@ -192,6 +192,27 @@ int o3db_smooth_bilateral(const float* positions_dev, const float* normals_dev, 
 int o3db_cluster_dbscan(const float* positions_dev /* [n,3] */, int64_t n, double eps, int64_t min_points,
                         int32_t* labels_dev /* [n] */, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Farthest-point down-sampling — t::geometry::PointCloud::FarthestPointDownSample
+ * (t/geometry/PointCloud.cpp:612-648); Float32.  selected_dev [num_samples] receives the
+ * selected indices in selection order, the result of this loop bit for bit (DESIGN.md §4.20):
+ *   d[j] = +inf for all j;  f = start_index
+ *   repeat num_samples times:
+ *       select f
+ *       for all j: e = ((dx*dx + dy*dy) + dz*dz), dx = x_j - x_f etc., all f32, each op
+ *                  rounded, no FMA (upstream's diff, diff * diff and Sum({1}));  d[j] = min(d[j], e)
+ *       f = argmax over the points not yet selected of d[j]; ties go to the lowest index
+ *           (the rule of the legacy geometry/PointCloud.cpp:543-554, strict >)
+ * Unlike upstream, a cloud with fewer distinct positions than num_samples still gives
+ * num_samples distinct indices (DESIGN.md §7).  Upstream returns the selected points in
+ * ascending index order; sort the indices to get that order.
+ * Errors, before any CUDA call: null pointers, n < 0 or n >= INT_MAX, num_samples < 1 or
+ * > n, start_index outside [0, n); after the launch: a non-finite coordinate (selected_dev
+ * is then unspecified).  One cooperative launch, one grid-wide barrier per sample; the call
+ * synchronises the stream once, to read the non-finite flag. */
+int o3db_farthest_point_down_sample(const float* positions_dev /* [n,3] */, int64_t n, int64_t num_samples,
+                                    int64_t start_index, int32_t* selected_dev /* [num_samples] */, void* stream);
+
 /* Reference-layout CSR spatial hash (parity / interop only): exactly the tables
  * BuildSpatialHashTableCUDA produces — cell = floor(p/(2r)), bucket =
  * SpatialHash(cell) % hash_table_size (core/nns/NeighborSearchCommon.h:31-52),

@@ -82,6 +82,7 @@ _SIGS = {
     "o3db_smooth_mls": (_i, [_vp, _i64, _dbl, _i, _vp, _vp, _vp]),
     "o3db_smooth_bilateral": (_i, [_vp, _vp, _i64, _dbl, _i, _dbl, _dbl, _vp, _vp]),
     "o3db_cluster_dbscan": (_i, [_vp, _i64, _dbl, _i64, _vp, _vp]),
+    "o3db_farthest_point_down_sample": (_i, [_vp, _i64, _i64, _i64, _vp, _vp]),
     "o3db_compute_pose_point_to_plane": (_i, [_vp, _vp, _vp, _vp, _i64, C.POINTER(RobustKernel), _vp, _vp,
                                               C.POINTER(_f), C.POINTER(_i), _vp]),
     "o3db_compute_pose_colored_icp": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(RobustKernel), _dbl,

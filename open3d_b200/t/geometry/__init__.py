@@ -365,6 +365,35 @@ class PointCloud:
                                       current_stream_ptr()))
         return labels
 
+    def farthest_point_down_sample(self, num_samples, start_index=0):
+        """PointCloud::FarthestPointDownSample (t/geometry/PointCloud.cpp:612-648; pybind pointcloud.cpp:253-263) -> a
+        new PointCloud of num_samples points, in ascending index order with every attribute: starting at start_index,
+        each next point is the one farthest (upstream's f32 squared distance) from those already chosen, ties to the
+        lowest index.  The whole selection runs in one launch (o3db_farthest_point_down_sample).  num_samples == 0
+        gives an empty cloud and num_samples == len(cloud) a clone, before start_index is checked, as upstream."""
+        num_samples, start_index = int(num_samples), int(start_index)
+        if num_samples < 0 or start_index < 0:
+            # upstream's arguments are size_t, which its binding refuses to take from a negative int
+            raise RuntimeError(f"farthest_point_down_sample: num_samples and start_index must be non-negative (got "
+                               f"{num_samples}, {start_index})")
+        p = self._positions_f32("FarthestPointDownSample")
+        n = int(p.shape[0])
+        if num_samples == 0:
+            return PointCloud()
+        if num_samples == n:
+            return self.clone()
+        if num_samples > n:
+            raise RuntimeError(f"Illegal number of samples: {num_samples}, must <= point size: {n}")
+        if start_index >= n:
+            raise RuntimeError(f"Illegal start index: {start_index}, must <= point size: {n}")
+        selected = torch.empty((num_samples,), dtype=torch.int32, device=p.device)
+        check(lib.o3db_farthest_point_down_sample(p.data_ptr(), n, num_samples, start_index, selected.data_ptr(),
+                                                  current_stream_ptr()))
+        idx = torch.sort(selected).values.long()
+        out = PointCloud()
+        out.point = {k: v[idx] for k, v in self.point.items()}
+        return out
+
     def _smooth_knn(self, who, iterations, factors, max_nn, fixed):
         p = self._positions_f32(who)
         if iterations < 0:
