@@ -213,6 +213,49 @@ int o3db_cluster_dbscan(const float* positions_dev /* [n,3] */, int64_t n, doubl
 int o3db_farthest_point_down_sample(const float* positions_dev /* [n,3] */, int64_t n, int64_t num_samples,
                                     int64_t start_index, int32_t* selected_dev /* [num_samples] */, void* stream);
 
+/* ------------------------------------------------------------------------
+ * The library's process-global random engine, utility::random (utility/Random.cpp): one std::mt19937, seeded from
+ * std::random_device until o3db_random_seed sets it to std::mt19937(seed), as o3d.utility.random.seed does.  Every
+ * random operation of the library draws from it, under one mutex.
+ * o3db_random_sample_indices draws num_samples rows of sample_size distinct indices into out_host
+ * [num_samples][sample_size], upstream's RandomSampler<size_t> (geometry/PointCloudSegmentation.cpp:30-55): each
+ * index from std::uniform_int_distribution<size_t>(0, n-1), a repeat within a row redrawn.  Host only. */
+int o3db_random_seed(int seed);
+int o3db_random_sample_indices(int64_t n, int sample_size, int num_samples, int64_t* out_host);
+
+/* ------------------------------------------------------------------------
+ * RANSAC plane segmentation — geometry::PointCloud::SegmentPlane (geometry/PointCloudSegmentation.cpp:157-279), which
+ * t::geometry::PointCloud::SegmentPlane (t/geometry/PointCloud.cpp:1646-1666) runs on the host; Float32 positions.
+ * The result is that of upstream's function run on one thread (DESIGN.md §4.21):
+ *   samples     num_iterations rows drawn up front as o3db_random_sample_indices does, all of them however early the
+ *               loop stops;
+ *   hypotheses  in f64 from the f32 positions: ComputeTrianglePlane (geometry/TriangleMesh.cpp:1248-1262) for
+ *               ransac_n == 3, else GetPlaneFromPoints over the sample in sample order; (0,0,0,0) is skipped;
+ *   scoring     a point is an inlier when |(a*x + c*z) + (b*y + d)| < distance_threshold, f64, each op rounded, no FMA
+ *               (Eigen's packet order for Vector4d::dot); fitness = inliers / n; rmse = sqrt(error / inliers), error
+ *               the sum of the squared distances sequential over each tile of 1024 points in index order, then over
+ *               the tiles in order (upstream sums all points in one sequence; DESIGN.md §7);
+ *   selection   hypotheses in index order, skipped once evaluated > break; a better one has the higher fitness, or
+ *               the same and a lower rmse; each improvement sets break = size_t(min(log(1-p)/log(1-fitness^ransac_n),
+ *               num_iterations)), or 0 at fitness 1; evaluated counts the non-degenerate hypotheses not skipped;
+ *   result      inliers_dev [n] receives the K points within the threshold of the best hypothesis in ascending
+ *               order, *num_inliers = K; plane_dev [4] receives GetPlaneFromPoints over them, with the sums in the
+ *               tile order above.  With no valid hypothesis (num_iterations <= 0, every sample collinear, a threshold
+ *               <= 0) the plane is (0,0,0,0) and K = 0.
+ * stats (optional, host): the best hypothesis's index (-1 for none), the evaluated count, its fitness and rmse.
+ * Errors, before any CUDA call, with upstream's messages: probability outside (0, 1], ransac_n < 3, n < ransac_n;
+ * also null pointers, n >= INT_MAX, num_iterations * ransac_n >= 2^31.  The call synchronises the stream once. */
+typedef struct {
+    int64_t best_index;
+    int64_t evaluated;
+    double fitness;
+    double inlier_rmse;
+} o3db_segment_stats;
+
+int o3db_segment_plane(const float* positions_dev /* [n,3] */, int64_t n, double distance_threshold, int ransac_n,
+                       int num_iterations, double probability, double* plane_dev /* [4] */,
+                       int64_t* inliers_dev /* [n] */, int64_t* num_inliers, o3db_segment_stats* stats, void* stream);
+
 /* Reference-layout CSR spatial hash (parity / interop only): exactly the tables
  * BuildSpatialHashTableCUDA produces — cell = floor(p/(2r)), bucket =
  * SpatialHash(cell) % hash_table_size (core/nns/NeighborSearchCommon.h:31-52),

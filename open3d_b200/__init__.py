@@ -11,6 +11,6 @@ for that path (same names, argument meaning and error behaviour as
 ``open3d.core.Tensor``.  There is no CPU fallback.
 """
 from . import _lib  # noqa: F401  (fails loudly if the shared library is missing)
-from . import core, t  # noqa: F401
+from . import core, t, utility  # noqa: F401
 
 __version__ = "0.1.0"

@@ -52,6 +52,11 @@ class OdometryResult(C.Structure):
                 ("status", C.c_int), ("iterations", C.c_int)]
 
 
+class SegmentStats(C.Structure):
+    _fields_ = [("best_index", C.c_int64), ("evaluated", C.c_int64), ("fitness", C.c_double),
+                ("inlier_rmse", C.c_double)]
+
+
 class RaycastOutputs(C.Structure):
     """o3db_raycast_outputs: device pointers, None = attribute not requested"""
     _fields_ = [(n, C.c_void_p) for n in ("depth", "vertex", "color", "normal", "index", "mask", "interp_ratio",
@@ -83,6 +88,10 @@ _SIGS = {
     "o3db_smooth_bilateral": (_i, [_vp, _vp, _i64, _dbl, _i, _dbl, _dbl, _vp, _vp]),
     "o3db_cluster_dbscan": (_i, [_vp, _i64, _dbl, _i64, _vp, _vp]),
     "o3db_farthest_point_down_sample": (_i, [_vp, _i64, _i64, _i64, _vp, _vp]),
+    "o3db_random_seed": (_i, [_i]),
+    "o3db_random_sample_indices": (_i, [_i64, _i, _i, _vp]),
+    "o3db_segment_plane": (_i, [_vp, _i64, _dbl, _i, _i, _dbl, _vp, _vp, C.POINTER(_i64), C.POINTER(SegmentStats),
+                                _vp]),
     "o3db_compute_pose_point_to_plane": (_i, [_vp, _vp, _vp, _vp, _i64, C.POINTER(RobustKernel), _vp, _vp,
                                               C.POINTER(_f), C.POINTER(_i), _vp]),
     "o3db_compute_pose_colored_icp": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(RobustKernel), _dbl,

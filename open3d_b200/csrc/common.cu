@@ -18,6 +18,16 @@ void set_last_error(const char* fmt, ...) {
 
 const char* last_error() { return g_last_error; }
 
+std::mt19937& random_engine() {
+    static std::mt19937 engine((int)std::random_device{}());   // upstream's Seed(rd()) takes an int
+    return engine;
+}
+
+std::mutex& random_mutex() {
+    static std::mutex mu;
+    return mu;
+}
+
 int alloc_failed(cudaError_t e, size_t bytes) {
     (void)cudaGetLastError();
     set_last_error("device allocation of %zu bytes failed: %s", bytes, cudaGetErrorString(e));

@@ -11,6 +11,8 @@
 #include <cstdio>
 #include <cstring>
 #include <memory>
+#include <mutex>
+#include <random>
 #include <type_traits>
 
 #include "../../include/open3d_b200.h"
@@ -63,6 +65,12 @@ inline int num_sms() {
 }
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// The library's one process-global random engine, utility::random's RandomContext (utility/Random.cpp:15-50): seeded
+// from std::random_device until o3db_random_seed replaces it with std::mt19937(seed).  Hold random_mutex() while
+// drawing from it.
+std::mt19937& random_engine();
+std::mutex& random_mutex();
 
 // Keep freed stream-ordered allocations cached in the device's default memory pool (the
 // default release threshold of 0 hands everything back to the driver at every synchronise,

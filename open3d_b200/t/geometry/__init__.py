@@ -365,6 +365,29 @@ class PointCloud:
                                       current_stream_ptr()))
         return labels
 
+    def segment_plane(self, distance_threshold=0.01, ransac_n=3, num_iterations=100, probability=0.999):
+        """PointCloud::SegmentPlane (t/geometry/PointCloud.cpp:1646-1666, geometry/PointCloudSegmentation.cpp:157-279;
+        pybind pointcloud.cpp:575-577) -> (plane_model, inliers) on the cloud's device: a torch.float64 [4] plane
+        (a, b, c, d) with a*x + b*y + c*z + d = 0, and the torch.int64 indices of its inliers in ascending order.
+        RANSAC over num_iterations samples of ransac_n points drawn from the library's random engine
+        (open3d_b200.utility.random.seed), stopping early by upstream's rule for the given probability; the result is
+        that of upstream's function run on one thread (o3db_segment_plane).  With no valid hypothesis the plane is
+        (0, 0, 0, 0) and there are no inliers."""
+        p = self._positions_f32("SegmentPlane")
+        n = int(p.shape[0])
+        ransac_n, num_iterations = int(ransac_n), int(num_iterations)
+        for name, v in (("ransac_n", ransac_n), ("num_iterations", num_iterations)):
+            if not -2 ** 31 <= v < 2 ** 31:
+                # upstream's arguments are C ints, which its binding refuses to take from a larger int
+                raise TypeError(f"segment_plane: {name} must fit in a 32-bit int (got {v})")
+        plane = torch.empty((4,), dtype=torch.float64, device=p.device)
+        inliers = torch.empty((max(n, 1),), dtype=torch.int64, device=p.device)
+        k = C.c_int64()
+        check(lib.o3db_segment_plane(p.data_ptr(), n, float(distance_threshold), ransac_n, num_iterations,
+                                     float(probability), plane.data_ptr(), inliers.data_ptr(), C.byref(k), None,
+                                     current_stream_ptr()))
+        return plane, inliers[:k.value].clone()
+
     def farthest_point_down_sample(self, num_samples, start_index=0):
         """PointCloud::FarthestPointDownSample (t/geometry/PointCloud.cpp:612-648; pybind pointcloud.cpp:253-263) -> a
         new PointCloud of num_samples points, in ascending index order with every attribute: starting at start_index,
