@@ -411,6 +411,19 @@ int o3db_orient_normals_to_align_with_direction(float* normals_dev, int64_t n, c
 int o3db_orient_normals_towards_camera_location(const float* positions_dev, float* normals_dev, int64_t n,
                                                 const float camera_host[3], void* stream);
 
+/* t::geometry::PointCloud::ComputeBoundaryPoints (t/geometry/PointCloud.cpp:803-853, kernel/PointCloudImpl.h:354-506):
+ * the hybrid search of the cloud on itself (radius > 0 and finite, max_nn in 1..32; upstream's default is 30); the
+ * first entry of each neighbour list is dropped as the point itself; the other m neighbours' angles in the plane of
+ * the point's normal are sorted, and mask_dev[i] = 1 where the largest gap between consecutive angles, the wrap-around
+ * included, exceeds angle_threshold degrees.  The frame and the dot products are f32 in upstream's order with no FMA;
+ * atan2 is evaluated in f64 and rounded to f32 (DESIGN.md §4.22).  m == 0 gives 0.  A normal whose frame is NaN
+ * (exactly (0,0,±1), zero, or a NaN component) gives a largest gap of 0, as upstream.
+ * max_gap_dev ([n] or NULL) receives each point's largest gap in radians (0 where m == 0).  Non-finite positions and
+ * infinite normal components return O3DB_ERR_INVALID.  n == 0 is a no-op.  Synchronises the stream. */
+int o3db_compute_boundary_points(const float* positions_dev, const float* normals_dev /* [n,3] */, int64_t n,
+                                 double radius, int max_nn, double angle_threshold, uint8_t* mask_dev /* [n] */,
+                                 float* max_gap_dev /* [n] or NULL */, void* stream);
+
 /* ------------------------------------------------------------------------
  * Fused, device-resident ICP loop — replaces
  * t::pipelines::registration::ICP / MultiScaleICP / DoSingleScaleICPIterations /

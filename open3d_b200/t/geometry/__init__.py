@@ -167,6 +167,35 @@ class PointCloud:
         self.point["normals"] = nrm
         return self
 
+    def compute_boundary_points(self, radius, max_nn=30, angle_threshold=90.0):
+        """PointCloud::ComputeBoundaryPoints (t/geometry/PointCloud.cpp:803-853; pybind pointcloud.cpp:628-651) ->
+        (PointCloud, mask): a point is on the boundary when the largest angular gap between its hybrid-search
+        neighbours (radius, max_nn in 1..32), seen in the plane of its normal, exceeds angle_threshold degrees.  The
+        mask is a torch.bool [n] on the device; every attribute is selected by it in the original order.  As upstream,
+        the first neighbour of each list is taken to be the point itself, and a normal of exactly (0, 0, +-1), a zero
+        normal or a NaN normal gives a NaN plane frame and never a boundary point (for angle_threshold >= 0), so an
+        exactly z-facing plane has no boundary.  Non-finite positions and infinite normal components raise.  An empty
+        cloud gives an empty cloud and an empty mask."""
+        p = self._positions_f32("ComputeBoundaryPoints")
+        n = int(p.shape[0])
+        if n > 0 and not self.has_point_normals():
+            raise RuntimeError("PointCloud must have normals attribute to compute boundary points.")
+        radius, max_nn = float(radius), int(max_nn)
+        if not radius > 0:
+            raise RuntimeError(f"ComputeBoundaryPoints: radius must be positive (got {radius})")
+        if not 1 <= max_nn <= 32:
+            raise RuntimeError(f"ComputeBoundaryPoints: max_nn must be in 1..32, the hybrid search's limit (got "
+                               f"{max_nn})")
+        mask = torch.zeros((n,), dtype=torch.bool, device=p.device)
+        if n > 0:
+            nrm = self._normals_f32(n)
+            check(lib.o3db_compute_boundary_points(p.data_ptr(), nrm.data_ptr(), n, radius, max_nn,
+                                                   float(angle_threshold), mask.data_ptr(), None,
+                                                   current_stream_ptr()))
+        out = PointCloud()
+        out.point = {k: v[mask] for k, v in self.point.items()}
+        return out, mask
+
     @staticmethod
     def create_from_depth_image(depth, intrinsics, extrinsics=None, depth_scale=1000.0, depth_max=3.0, stride=1,
                                 with_normals=False):
