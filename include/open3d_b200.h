@@ -424,6 +424,27 @@ int o3db_compute_boundary_points(const float* positions_dev, const float* normal
                                  double radius, int max_nn, double angle_threshold, uint8_t* mask_dev /* [n] */,
                                  float* max_gap_dev /* [n] or NULL */, void* stream);
 
+/* t::geometry::PointCloud::RemoveRadiusOutliers (t/geometry/PointCloud.cpp:650-676): mask_dev[i] = 1 when at least
+ * nb_points points, point i included, lie within search_radius of it, with the predicate of upstream's CUDA radius
+ * search: d = p - q in f32, dist = fma(d2, d2, fma(d1, d1, fma(d0, d0, 0))), a neighbour iff dist <= r * r, r the
+ * radius rounded to f32 (DESIGN.md §4.23).  nb_points < 1 or search_radius <= 0 give upstream's error; a NaN or
+ * infinite radius and non-finite positions return O3DB_ERR_INVALID.  nb_points > n keeps nothing.  n == 0 is a
+ * no-op.  Synchronises the stream once, for the index's bounding box. */
+int o3db_remove_radius_outliers(const float* positions_dev /* [n,3] */, int64_t n, int64_t nb_points,
+                                double search_radius, uint8_t* mask_dev /* [n] */, void* stream);
+
+/* t::geometry::PointCloud::RemoveDuplicatedPoints (t/geometry/PointCloud.cpp:740-760): two points are duplicates when
+ * their coordinates are equal bit for bit (so -0.0 != 0.0, and NaNs with equal bits are duplicates); mask_dev[i] = 1
+ * for the lowest index of each group.  Any bit pattern is accepted.  n == 0 is a no-op.  Does not synchronise. */
+int o3db_remove_duplicated_points(const float* positions_dev /* [n,3] */, int64_t n, uint8_t* mask_dev /* [n] */,
+                                  void* stream);
+
+/* t::geometry::PointCloud::RemoveNonFinitePoints (t/geometry/PointCloud.cpp:716-738): mask_dev[i] = 0 when remove_nan
+ * and a coordinate is NaN, or remove_inf and a coordinate is infinite; 1 otherwise.  n == 0 is a no-op.  Does not
+ * synchronise. */
+int o3db_remove_non_finite_points(const float* positions_dev /* [n,3] */, int64_t n, int remove_nan, int remove_inf,
+                                  uint8_t* mask_dev /* [n] */, void* stream);
+
 /* ------------------------------------------------------------------------
  * Fused, device-resident ICP loop — replaces
  * t::pipelines::registration::ICP / MultiScaleICP / DoSingleScaleICPIterations /

@@ -108,6 +108,9 @@ _SIGS = {
     "o3db_orient_normals_to_align_with_direction": (_i, [_vp, _i64, _vp, _vp]),
     "o3db_orient_normals_towards_camera_location": (_i, [_vp, _vp, _i64, _vp, _vp]),
     "o3db_compute_boundary_points": (_i, [_vp, _vp, _i64, _dbl, _i, _dbl, _vp, _vp, _vp]),
+    "o3db_remove_radius_outliers": (_i, [_vp, _i64, _i64, _dbl, _vp, _vp]),
+    "o3db_remove_duplicated_points": (_i, [_vp, _i64, _vp, _vp]),
+    "o3db_remove_non_finite_points": (_i, [_vp, _i64, _i, _i, _vp, _vp]),
     "o3db_icp_create_colored": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions), _dbl, _vp,
                                      _vp, C.POINTER(_vp)]),
     "o3db_icp_colored": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions), _dbl,

@@ -18,13 +18,10 @@
 
 namespace o3db {
 
-// What the neighbour passes read: the sorted table, the binning radius and upstream's squared radius.
+// What the neighbour passes read: the sorted table with its binning radius, and upstream's squared radius.
 struct DbscanView {
-    Grid g;
-    const float4* pts;    // sorted positions, .w = original index bits
-    const unsigned* cs;   // cell_start
-    float rr;             // eps, rounded up a little: the box [q - rr, q + rr] holds every neighbour of q
-    double eps2;          // eps * eps in f64, as KDTreeFlann::SearchRadius passes it to nanoflann
+    RadiusView box;   // box.rr = eps, rounded up a little
+    double eps2;      // eps * eps in f64, as KDTreeFlann::SearchRadius passes it to nanoflann
 };
 
 // nanoflann's L2_Adaptor::evalMetric for dimension 3 and RadiusResultSet::addPoint: d2 = ((0 + dx dx) + dy dy) + dz dz
@@ -37,26 +34,10 @@ __device__ __forceinline__ bool dbscan_neighbour(const float4 q, const float4 p,
     return d2 < eps2;
 }
 
-// Calls f(slot) for every neighbour of q at a sorted slot >= from, in slot order within each row of cells, until f
-// returns false.  The cells are those binned from [q - rr, q + rr] along each grid axis: binning is monotone and
-// lo_bound / hi_bound widen the box by more than the rounding of its ends, so no neighbour lies outside them.
+// radius_visit (grid.cuh) with upstream's predicate: f(slot) for every neighbour of q at a sorted slot >= from.
 template <typename F>
 __device__ __forceinline__ void dbscan_visit(const DbscanView& v, const float4 q, unsigned from, F&& f) {
-    float gx, gy, gz;
-    to_grid(v.g, q.x, q.y, q.z, gx, gy, gz);
-    const int x0 = cell1(lo_bound(gx, v.rr), v.g.ox, v.g.inv_cx, v.g.nx);
-    const int x1 = cell1(hi_bound(gx, v.rr), v.g.ox, v.g.inv_cx, v.g.nx);
-    const int y0 = cell1(lo_bound(gy, v.rr), v.g.oy, v.g.inv_c, v.g.ny);
-    const int y1 = cell1(hi_bound(gy, v.rr), v.g.oy, v.g.inv_c, v.g.ny);
-    const int z0 = cell1(lo_bound(gz, v.rr), v.g.oz, v.g.inv_c, v.g.nz);
-    const int z1 = cell1(hi_bound(gz, v.rr), v.g.oz, v.g.inv_c, v.g.nz);
-    for (int iz = z0; iz <= z1; ++iz)
-        for (int iy = y0; iy <= y1; ++iy) {
-            const int row = (iz * v.g.ny + iy) * v.g.nx;
-            const unsigned e = __ldg(&v.cs[row + x1 + 1]);
-            for (unsigned j = max(__ldg(&v.cs[row + x0]), from); j < e; ++j)
-                if (dbscan_neighbour(q, __ldg(&v.pts[j]), v.eps2) && !f(j)) return;
-        }
+    radius_visit(v.box, q, from, [&](const float4 p) { return dbscan_neighbour(q, p, v.eps2); }, f);
 }
 
 // The root of x's tree.  Every parent is an ancestor at a lower slot, so path halving (a plain store of the
@@ -97,7 +78,7 @@ __global__ void __launch_bounds__(kThreads) dbscan_core_kernel(DbscanView v, int
     if (s >= n) return;
     int count = 0;
     if (need > 0)
-        dbscan_visit(v, __ldg(&v.pts[s]), 0u, [&](unsigned) { return ++count < need; });
+        dbscan_visit(v, __ldg(&v.box.pts[s]), 0u, [&](unsigned) { return ++count < need; });
     core[s] = count >= need;
     parent[s] = (unsigned)s;
     cmin[s] = 0xffffffffu;
@@ -108,7 +89,7 @@ __global__ void __launch_bounds__(kThreads) dbscan_union_kernel(DbscanView v, in
                                                                 const uint8_t* __restrict__ core, unsigned* parent) {
     const int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (s >= n || !core[s]) return;
-    dbscan_visit(v, __ldg(&v.pts[s]), (unsigned)s + 1u, [&](unsigned j) {
+    dbscan_visit(v, __ldg(&v.box.pts[s]), (unsigned)s + 1u, [&](unsigned j) {
         if (core[j]) dbscan_unite(parent, (unsigned)s, j);
         return true;
     });
@@ -147,7 +128,7 @@ __global__ void __launch_bounds__(kThreads) dbscan_label_kernel(DbscanView v, in
                                                                 int32_t* __restrict__ labels) {
     const int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (s >= n) return;
-    const float4 q = __ldg(&v.pts[s]);
+    const float4 q = __ldg(&v.box.pts[s]);
     unsigned best = 0xffffffffu;
     if (core[s]) {
         best = id[cmin[root[s]]];
@@ -160,44 +141,11 @@ __global__ void __launch_bounds__(kThreads) dbscan_label_kernel(DbscanView v, in
     labels[__float_as_int(q.w)] = best == 0xffffffffu ? -1 : (int32_t)best;
 }
 
-// nonfinite = 1 when any coordinate is NaN or infinite (bbox_kernel's fminf / fmaxf skip NaN)
+// nonfinite = 1 when any coordinate is NaN or infinite (grid_index_finite)
 __global__ void __launch_bounds__(kThreads) dbscan_finite_kernel(const float* __restrict__ pts, int64_t n,
                                                                  unsigned* __restrict__ nonfinite) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    if (!isfinite(pts[3 * i]) || !isfinite(pts[3 * i + 1]) || !isfinite(pts[3 * i + 2])) atomicOr(nonfinite, 1u);
-}
-
-struct DbscanBox {
-    unsigned bbox[6];
-    unsigned nonfinite;
-};
-
-// The cell-sorted table of the cloud, cells of at least eps.  Synchronises st once, for the bounding box.
-static int dbscan_index(o3db_nns* s, const float* pts, int64_t n, double eps, cudaStream_t st) {
-    configure_memory_pool();
-    s->stream = st;
-    s->m = n;
-    s->radius = eps;
-    DbscanBox h{};
-    {
-        DevPtr<DbscanBox> d;
-        if (int rc = dev_alloc(d, 1, st)) return rc;
-        O3DB_CUDA_CHECK(cudaMemsetAsync(&d->nonfinite, 0, sizeof(unsigned), st));
-        if (int rc = bbox_launch(pts, n, d->bbox, st)) return rc;
-        dbscan_finite_kernel<<<(unsigned)ceil_div(n, kThreads), kThreads, 0, st>>>(pts, n, &d->nonfinite);
-        O3DB_LAUNCH_CHECK();
-        O3DB_CUDA_CHECK(cudaMemcpyAsync(&h, d.get(), sizeof(h), cudaMemcpyDeviceToHost, st));
-        O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
-    }
-    float mn[3], mx[3];
-    if (bbox_decode(h.bbox, mn, mx) || h.nonfinite) {
-        set_last_error("ClusterDBSCAN: the point cloud has non-finite coordinates");
-        return O3DB_ERR_INVALID;
-    }
-    // without thin cells: cells of eps (1 + 1e-4), grown by grid_from_bbox where the cloud's extent needs it
-    grid_from_bbox(mn, mx, eps * (1.0 + 1e-4), false, n, &s->g, &s->ncell);
-    return grid_sort(s, pts, nullptr, n, st);
+    if (i < n) flag_nonfinite(pts, i, nonfinite);
 }
 
 }  // namespace o3db
@@ -215,10 +163,12 @@ int o3db_cluster_dbscan(const float* positions_dev, int64_t n, double eps, int64
     if (n == 0) return O3DB_OK;
     cudaStream_t st = (cudaStream_t)stream;
     o3db_nns index;
-    if (int rc = dbscan_index(&index, positions_dev, n, eps, st)) return rc;
+    if (int rc = grid_index_finite(&index, positions_dev, n, eps, dbscan_finite_kernel,
+                                   "ClusterDBSCAN: the point cloud has non-finite coordinates", st))
+        return rc;
     // rr >= eps after its rounding to f32; an eps beyond the f32 range bins every point into the box
     const double rr = eps * (1.0 + 1e-5);
-    const DbscanView v{index.g, index.pts4.get(), index.cell_start.get(), rr < (double)FLT_MAX ? (float)rr : INFINITY,
+    const DbscanView v{{index.g, index.pts4.get(), index.cell_start.get(), rr < (double)FLT_MAX ? (float)rr : INFINITY},
                        eps * eps};
     DevPtr<uint8_t> core;
     DevPtr<unsigned> parent, root, cmin, id, scratch;
@@ -236,7 +186,7 @@ int o3db_cluster_dbscan(const float* positions_dev, int64_t n, double eps, int64
     O3DB_LAUNCH_CHECK();
     dbscan_union_kernel<<<nb, kThreads, 0, st>>>(v, n, core.get(), parent.get());
     O3DB_LAUNCH_CHECK();
-    dbscan_flatten_kernel<<<nb, kThreads, 0, st>>>(v.pts, n, core.get(), parent.get(), root.get(), cmin.get());
+    dbscan_flatten_kernel<<<nb, kThreads, 0, st>>>(v.box.pts, n, core.get(), parent.get(), root.get(), cmin.get());
     O3DB_LAUNCH_CHECK();
     dbscan_root_flag_kernel<<<nb, kThreads, 0, st>>>(n, core.get(), root.get(), cmin.get(), id.get());
     O3DB_LAUNCH_CHECK();

@@ -60,6 +60,20 @@ int bbox_decode(const unsigned h_bbox[6], float mn[3], float mx[3]);
 void grid_from_bbox(const float mn[3], const float mx[3], double c, bool thin_cells, int64_t m, Grid* g, int64_t* ncell);
 int grid_sort(o3db_nns* s, const float* pts, const float* nrm, int64_t m, cudaStream_t st);
 
+// The index of the calls that reject non-finite coordinates (DBSCAN, the radius-outlier count): the bounding box and
+// `finite` (which sets its flag for a NaN or infinite coordinate, see flag_nonfinite) on st, one synchronise, then
+// cells of radius (1 + 1e-4) without thin cells, grown by grid_from_bbox where the cloud's extent needs it.  A flagged
+// cloud sets `nonfinite_msg` as the last error and returns O3DB_ERR_INVALID.  `finite` is the caller's own kernel, so
+// that each call's kernels keep their names in a trace.
+using FiniteKernel = void (*)(const float*, int64_t, unsigned*);
+int grid_index_finite(o3db_nns* s, const float* pts, int64_t n, double radius, FiniteKernel finite,
+                      const char* nonfinite_msg, cudaStream_t st);
+
+// *flag = 1 when a coordinate of point i is NaN or infinite (bbox_kernel's fminf / fmaxf skip NaN)
+__device__ __forceinline__ void flag_nonfinite(const float* __restrict__ pts, int64_t i, unsigned* flag) {
+    if (!isfinite(pts[3 * i]) || !isfinite(pts[3 * i + 1]) || !isfinite(pts[3 * i + 2])) atomicOr(flag, 1u);
+}
+
 __device__ __forceinline__ float pick_axis(int a, float x, float y, float z) { return a == 0 ? x : (a == 1 ? y : z); }
 // real (x,y,z) -> grid-ordered (gx,gy,gz)
 __device__ __forceinline__ void to_grid(const Grid& g, float x, float y, float z, float& gx, float& gy, float& gz) {
@@ -89,6 +103,37 @@ __device__ __forceinline__ unsigned cell_key(const Grid& g, float rx, float ry, 
 // given that dist^2 was accepted in f32: r' = r (1 + 1e-6) plus 2 ulp of |q|.
 __device__ __forceinline__ float lo_bound(float q, float rr) { return (q - rr) - fabsf(q) * 2.4e-7f; }
 __device__ __forceinline__ float hi_bound(float q, float rr) { return (q + rr) + fabsf(q) * 2.4e-7f; }
+
+// A cell-sorted table searched by radius (grid_index_finite): every neighbour of q lies in the cells binned from
+// [q - rr, q + rr] along each grid axis.
+struct RadiusView {
+    Grid g;
+    const float4* pts;    // sorted positions, .w = original index bits
+    const unsigned* cs;   // cell_start
+    float rr;             // the radius, rounded up a little: the box [q - rr, q + rr] holds every neighbour of q
+};
+
+// Calls f(slot) for every slot >= from whose point p passes near(p), in slot order within each row of cells, until f
+// returns false.  The cells are those binned from [q - rr, q + rr] along each grid axis: binning is monotone and
+// lo_bound / hi_bound widen the box by more than the rounding of its ends, so no neighbour lies outside them.
+template <typename P, typename F>
+__device__ __forceinline__ void radius_visit(const RadiusView& v, const float4 q, unsigned from, P&& near, F&& f) {
+    float gx, gy, gz;
+    to_grid(v.g, q.x, q.y, q.z, gx, gy, gz);
+    const int x0 = cell1(lo_bound(gx, v.rr), v.g.ox, v.g.inv_cx, v.g.nx);
+    const int x1 = cell1(hi_bound(gx, v.rr), v.g.ox, v.g.inv_cx, v.g.nx);
+    const int y0 = cell1(lo_bound(gy, v.rr), v.g.oy, v.g.inv_c, v.g.ny);
+    const int y1 = cell1(hi_bound(gy, v.rr), v.g.oy, v.g.inv_c, v.g.ny);
+    const int z0 = cell1(lo_bound(gz, v.rr), v.g.oz, v.g.inv_c, v.g.nz);
+    const int z1 = cell1(hi_bound(gz, v.rr), v.g.oz, v.g.inv_c, v.g.nz);
+    for (int iz = z0; iz <= z1; ++iz)
+        for (int iy = y0; iy <= y1; ++iy) {
+            const int row = (iz * v.g.ny + iy) * v.g.nx;
+            const unsigned e = __ldg(&v.cs[row + x1 + 1]);
+            for (unsigned j = max(__ldg(&v.cs[row + x0]), from); j < e; ++j)
+                if (near(__ldg(&v.pts[j])) && !f(j)) return;
+        }
+}
 
 static constexpr unsigned kSlabMax = 32;   // longest slab scanned whole (see nn_search_two_pass)
 

@@ -444,6 +444,35 @@ int grid_sort(o3db_nns* s, const float* pts, const float* nrm, int64_t m, cudaSt
     return O3DB_OK;
 }
 
+int grid_index_finite(o3db_nns* s, const float* pts, int64_t n, double radius, FiniteKernel finite,
+                      const char* nonfinite_msg, cudaStream_t st) {
+    configure_memory_pool();
+    s->stream = st;
+    s->m = n;
+    s->radius = radius;
+    struct Probe {
+        unsigned bbox[6];
+        unsigned nonfinite;
+    } h{};
+    {
+        DevPtr<Probe> d;
+        if (int rc = dev_alloc(d, 1, st)) return rc;
+        O3DB_CUDA_CHECK(cudaMemsetAsync(&d->nonfinite, 0, sizeof(unsigned), st));
+        if (int rc = bbox_launch(pts, n, d->bbox, st)) return rc;
+        finite<<<(unsigned)ceil_div(n, kThreads), kThreads, 0, st>>>(pts, n, &d->nonfinite);
+        O3DB_LAUNCH_CHECK();
+        O3DB_CUDA_CHECK(cudaMemcpyAsync(&h, d.get(), sizeof(h), cudaMemcpyDeviceToHost, st));
+        O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
+    }
+    float mn[3], mx[3];
+    if (bbox_decode(h.bbox, mn, mx) || h.nonfinite) {
+        set_last_error("%s", nonfinite_msg);
+        return O3DB_ERR_INVALID;
+    }
+    grid_from_bbox(mn, mx, radius * (1.0 + 1e-4), false, n, &s->g, &s->ncell);
+    return grid_sort(s, pts, nullptr, n, st);
+}
+
 // Builds pts4 / nrm4 / cell_start for `pts` (device), cells of radius x cell_scale.  Synchronises `st` once
 // (the grid dimensions depend on the bounding box).
 static int nns_build(o3db_nns* s, const float* pts, const float* nrm, int64_t m, double radius,

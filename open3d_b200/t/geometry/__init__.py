@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import enum
+import math
 import weakref
 
 import numpy as np
@@ -310,6 +311,55 @@ class PointCloud:
         out = PointCloud()
         out.point = {k: v[mask] for k, v in self.point.items()}
         return out, mask
+
+    def remove_radius_outliers(self, nb_points, search_radius):
+        """PointCloud::RemoveRadiusOutliers (t/geometry/PointCloud.cpp:650-676; pybind pointcloud.cpp:264) ->
+        (PointCloud, mask): keeps the points with at least nb_points points, themselves included, within
+        search_radius, with the distance test of upstream's CUDA radius search (f32, dist <= radius^2).  The mask is a
+        torch.bool [n] on the device; every attribute is selected by it in the original order.  A NaN or infinite
+        radius raises, and so do non-finite positions (see remove_non_finite_points).  An empty cloud gives an empty
+        cloud and an empty mask."""
+        nb_points, search_radius = int(nb_points), float(search_radius)
+        if nb_points < 1 or search_radius <= 0:
+            raise RuntimeError("Illegal input parameters, number of points and radius must be positive")
+        if not math.isfinite(search_radius):
+            raise RuntimeError(f"RemoveRadiusOutliers: search_radius must be finite (got {search_radius})")
+        p = self._positions_f32("RemoveRadiusOutliers")
+        n = int(p.shape[0])
+        mask = torch.empty((n,), dtype=torch.bool, device=p.device)
+        if n > 0:
+            check(lib.o3db_remove_radius_outliers(p.data_ptr(), n, nb_points, search_radius, mask.data_ptr(),
+                                                  current_stream_ptr()))
+        return self._select(mask), mask
+
+    def remove_duplicated_points(self):
+        """PointCloud::RemoveDuplicatedPoints (t/geometry/PointCloud.cpp:740-760) -> (PointCloud, mask): of the points
+        whose three coordinates are equal bit for bit (so -0.0 and 0.0 differ, and NaNs with equal bits are equal), the
+        one with the lowest index is kept.  The mask is a torch.bool [n] on the device; every attribute is selected by
+        it in the original order."""
+        p = self._positions_f32("RemoveDuplicatedPoints")
+        n = int(p.shape[0])
+        mask = torch.empty((n,), dtype=torch.bool, device=p.device)
+        if n > 0:
+            check(lib.o3db_remove_duplicated_points(p.data_ptr(), n, mask.data_ptr(), current_stream_ptr()))
+        return self._select(mask), mask
+
+    def remove_non_finite_points(self, remove_nan=True, remove_inf=True):
+        """PointCloud::RemoveNonFinitePoints (t/geometry/PointCloud.cpp:716-738) -> (PointCloud, mask): removes the
+        points with a NaN coordinate when remove_nan and those with an infinite one when remove_inf.  The mask is a
+        torch.bool [n] on the device; every attribute is selected by it in the original order."""
+        p = self._positions_f32("RemoveNonFinitePoints")
+        n = int(p.shape[0])
+        mask = torch.empty((n,), dtype=torch.bool, device=p.device)
+        if n > 0:
+            check(lib.o3db_remove_non_finite_points(p.data_ptr(), n, int(bool(remove_nan)), int(bool(remove_inf)),
+                                                    mask.data_ptr(), current_stream_ptr()))
+        return self._select(mask), mask
+
+    def _select(self, mask):
+        out = PointCloud()
+        out.point = {k: v[mask] for k, v in self.point.items()}
+        return out
 
     def compute_metrics(self, pcd2, metrics, params=None):
         """PointCloud::ComputeMetrics (t/geometry/PointCloud.cpp:1805-1835, kernel/Metrics.cpp) -> a CPU Float32
