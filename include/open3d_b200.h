@@ -114,6 +114,15 @@ int o3db_knn_search(const o3db_knn* knn, const float* queries_dev /* [N,3] */, i
                     int index_dtype, void* indices_dev /* [N,k'] */, float* distances_dev /* [N,k'] */,
                     void* stream);
 
+/* The search FPFH's neighbour lists come from (DESIGN.md §4.24): the k' = min(knn, M) nearest dataset points of every
+ * query, knn in 1..128, with dist^2 <= (float)radius * (float)radius when radius > 0 (radius == 0: no cap), ascending
+ * by (dist^2, index).  indices_dev / distances_dev [N,k'] Int32 / Float32 get -1 / 0 past counts_dev [N].  For
+ * knn <= 32 and radius > 0 the lists equal o3db_nns_hybrid_search's; with radius == 0 they equal o3db_knn_search's.
+ * A query with a non-finite coordinate returns O3DB_ERR_INVALID; that check synchronises the stream once. */
+int o3db_knn_search_lists(const o3db_knn* knn, const float* queries_dev /* [N,3] */, int64_t num_queries, int knn_k,
+                          double radius, int32_t* indices_dev, float* distances_dev, int32_t* counts_dev,
+                          void* stream);
+
 /* The index's cell size, fine-cell count and coarse-block count (diagnostics). */
 int o3db_knn_index_stats(const o3db_knn* knn, double* cell_size, int64_t* num_cells, int64_t* num_blocks);
 
@@ -423,6 +432,31 @@ int o3db_orient_normals_towards_camera_location(const float* positions_dev, floa
 int o3db_compute_boundary_points(const float* positions_dev, const float* normals_dev /* [n,3] */, int64_t n,
                                  double radius, int max_nn, double angle_threshold, uint8_t* mask_dev /* [n] */,
                                  float* max_gap_dev /* [n] or NULL */, void* stream);
+
+/* t::pipelines::registration::ComputeFPFHFeature (t/pipelines/registration/Feature.cpp:23-277,
+ * kernel/FeatureImpl.h:23-293): the 33-bin FPFH feature of each point over its neighbour list, the min(max_nn, n)
+ * nearest points (max_nn in 4..128) capped at dist^2 <= (float)radius^2 when radius > 0 (the hybrid search), uncapped
+ * when radius == 0 (KNN only).  The first entry of each list is dropped as the point itself.  indices_dev ([num_indices]
+ * Int64, any order, repeats allowed) selects rows: fpfh_dev receives one row per distinct index in ascending point
+ * order, each equal to that point's row of the call without indices; num_indices == -1 selects every point.
+ * fpfh_dev holds [rows, 33]; *num_rows receives the row count.  Pair features are f32 in upstream's order with no FMA,
+ * acos / atan2 evaluated in f64 and rounded to f32 (DESIGN.md §4.24).  Non-finite positions or normal components and
+ * indices outside [0, n) return O3DB_ERR_INVALID.  n == 0 or num_indices == 0 gives no rows.  Synchronises the
+ * stream. */
+int o3db_compute_fpfh_feature(const float* positions_dev, const float* normals_dev /* [n,3] */, int64_t n, int max_nn,
+                              double radius, const int64_t* indices_dev, int64_t num_indices,
+                              float* fpfh_dev /* [rows,33] */, int64_t* num_rows, void* stream);
+
+/* t::pipelines::registration::CorrespondencesFromFeatures (t/pipelines/registration/Feature.cpp:279-333): for each
+ * source row i of [n, dim] the nearest target row of [m, dim] by the f32 sum over d of fmaf(s - t, s - t, acc), ties
+ * to the lowest index.  corres_dev ([n, 2] Int64) receives (i, nearest) rows; with mutual_filter only the rows whose
+ * target's nearest source is i, in source order, when there are more than mutual_consistent_ratio * n of them (f32, as
+ * upstream), else every row.  *num_corres receives the row count, *num_mutual (or NULL) the mutual count.  n == 0
+ * gives no rows; m == 0 with n > 0 returns O3DB_ERR_INVALID.  Synchronises the stream. */
+int o3db_correspondences_from_features(const float* source_dev /* [n,dim] */, int64_t n,
+                                       const float* target_dev /* [m,dim] */, int64_t m, int dim, int mutual_filter,
+                                       float mutual_consistent_ratio, int64_t* corres_dev /* [n,2] */,
+                                       int64_t* num_corres, int64_t* num_mutual, void* stream);
 
 /* t::geometry::PointCloud::RemoveRadiusOutliers (t/geometry/PointCloud.cpp:650-676): mask_dev[i] = 1 when at least
  * nb_points points, point i included, lie within search_radius of it, with the predicate of upstream's CUDA radius

@@ -80,6 +80,7 @@ _SIGS = {
     "o3db_knn_create": (_i, [_vp, _i64, _vp, C.POINTER(_vp)]),
     "o3db_knn_destroy": (None, [_vp]),
     "o3db_knn_search": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp, _vp]),
+    "o3db_knn_search_lists": (_i, [_vp, _vp, _i64, _i, _dbl, _vp, _vp, _vp, _vp]),
     "o3db_knn_index_stats": (_i, [_vp, _dp, C.POINTER(_i64), C.POINTER(_i64)]),
     "o3db_remove_statistical_outliers": (_i, [_vp, _i64, _i, _dbl, _vp, _vp, _vp]),
     "o3db_compute_metrics": (_i, [_vp, _i64, _vp, _i64, _vp, _i, _vp, _i, _vp, _i64, _vp]),
@@ -108,6 +109,9 @@ _SIGS = {
     "o3db_orient_normals_to_align_with_direction": (_i, [_vp, _i64, _vp, _vp]),
     "o3db_orient_normals_towards_camera_location": (_i, [_vp, _vp, _i64, _vp, _vp]),
     "o3db_compute_boundary_points": (_i, [_vp, _vp, _i64, _dbl, _i, _dbl, _vp, _vp, _vp]),
+    "o3db_compute_fpfh_feature": (_i, [_vp, _vp, _i64, _i, _dbl, _vp, _i64, _vp, C.POINTER(_i64), _vp]),
+    "o3db_correspondences_from_features": (_i, [_vp, _i64, _vp, _i64, _i, _i, _f, _vp, C.POINTER(_i64),
+                                                C.POINTER(_i64), _vp]),
     "o3db_remove_radius_outliers": (_i, [_vp, _i64, _i64, _dbl, _vp, _vp]),
     "o3db_remove_duplicated_points": (_i, [_vp, _i64, _vp, _vp]),
     "o3db_remove_non_finite_points": (_i, [_vp, _i64, _i, _i, _vp, _vp]),

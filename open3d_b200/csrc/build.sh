@@ -11,7 +11,7 @@ FLAGS=("${ARCH[@]}" -lineinfo -O3 -std=c++17
 cd "${HERE}"
 OBJS=()
 PIDS=()
-for f in common icp tsdf comm pointcloud raycast odometry extract projection knn smooth dbscan fps segment boundary remove; do
+for f in common icp tsdf comm pointcloud raycast odometry extract projection knn smooth dbscan fps segment boundary remove fpfh; do
   "${NVCC}" "${FLAGS[@]}" -c "${f}.cu" -o "${f}.o" &
   PIDS+=($!)
   OBJS+=("${f}.o")

@@ -69,6 +69,13 @@ using FiniteKernel = void (*)(const float*, int64_t, unsigned*);
 int grid_index_finite(o3db_nns* s, const float* pts, int64_t n, double radius, FiniteKernel finite,
                       const char* nonfinite_msg, cudaStream_t st);
 
+// knn.cu's wide search, FPFH's neighbour lists: for each of nq finite queries, the k' = min(k, M) nearest points of
+// the index with dist^2 <= thr (+inf: no cap), ascending by (dist^2, index), into idx / d2 [nq, k'] (-1 / 0 past the
+// count) and cnt [nq]; k in 1..kKnnWideMax.  With kp <= 32 the capped list equals o3db_nns_hybrid_search's.
+static constexpr int kKnnWideMax = 128;
+int knn_lists(const o3db_knn* knn, const float* queries, int64_t nq, int k, float thr, int32_t* idx, float* d2,
+              int32_t* cnt, cudaStream_t st);
+
 // *flag = 1 when a coordinate of point i is NaN or infinite (bbox_kernel's fminf / fmaxf skip NaN)
 __device__ __forceinline__ void flag_nonfinite(const float* __restrict__ pts, int64_t i, unsigned* flag) {
     if (!isfinite(pts[3 * i]) || !isfinite(pts[3 * i + 1]) || !isfinite(pts[3 * i + 2])) atomicOr(flag, 1u);

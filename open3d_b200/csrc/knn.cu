@@ -1,6 +1,7 @@
 // knn.cu — exact k-nearest-neighbour search (k <= 32) over a cell-sorted index, and its two consumers on the
 // device: PointCloud::RemoveStatisticalOutliers and PointCloud::ComputeMetrics.  See include/open3d_b200.h for the
-// reference functions each entry point replaces and DESIGN.md §4.17 for the design.
+// reference functions each entry point replaces and DESIGN.md §4.17 for the design.  The same walk with a list of up to
+// 128 keys and an optional radius cap gives FPFH its neighbour lists (knn_lists, DESIGN.md §4.24).
 #include <cfloat>
 #include <cstddef>
 #include <climits>
@@ -15,6 +16,7 @@
 namespace o3db {
 
 static constexpr int kKnnMax = 32;
+static_assert(kKnnWideMax == 4 * 32, "knn_lists' list holds four keys per lane");
 static constexpr int kBlockShift = 3;           // a coarse block is 8 x 8 x 8 fine cells
 static constexpr int kOccLevels = 8;            // cell sizes c0 * 2^L probed for their occupancy
 static constexpr unsigned kOccCells = 1u << 24; // cells of probe level 0 at most (a 2 MB bitmap per level)
@@ -180,32 +182,90 @@ __device__ __forceinline__ void knn_offer(unsigned long long& key, int kp, unsig
     }
 }
 
+// The list of knn_search_kernel: one key per lane, k <= 32.
+struct KnnList {
+    unsigned long long key = ~0ull;
+    int kp;
+    __device__ __forceinline__ float bound() const { return kth_dist2(key, kp); }
+    __device__ __forceinline__ bool accept(float) const { return true; }
+    __device__ __forceinline__ void offer(unsigned long long cand) { knn_offer(key, kp, cand); }
+};
+
+// The list of knn_lists_kernel: four keys per lane, k <= 128.  Slot s of lane j holds the (32 s + j)-th smallest key;
+// slots above `last` = (kp - 1) / 32 stay ~0 and are never read.  A candidate beyond the cap (dist^2 > thr, +inf for
+// none) is not offered, and the pruning bound is min(k-th dist^2, thr): while fewer than kp keys are held the k-th is
+// the NaN 0xffffffff, and fminf then gives thr.  The slots are four named registers: an array indexed by `last` would
+// be placed in local memory.
+struct KnnWideList {
+    unsigned long long k0 = ~0ull, k1 = ~0ull, k2 = ~0ull, k3 = ~0ull;
+    int kp, last;
+    float thr;
+    __device__ __forceinline__ KnnWideList(int kp_, float thr_) : kp(kp_), last((kp_ - 1) >> 5), thr(thr_) {}
+    __device__ __forceinline__ unsigned long long kth_key() const {
+        return __shfl_sync(kFull, last == 0 ? k0 : (last == 1 ? k1 : (last == 2 ? k2 : k3)), (kp - 1) & 31);
+    }
+    __device__ __forceinline__ float bound() const { return fminf(__uint_as_float((unsigned)(kth_key() >> 32)), thr); }
+    __device__ __forceinline__ bool accept(float d) const { return d <= thr; }
+    // slot s (base 32 s) after inserting c at position pos; carry is lane 31 of slot s - 1 before the insertion
+    static __device__ __forceinline__ void shift(unsigned long long& k, int base, unsigned long long carry,
+                                                 unsigned long long c, int pos) {
+        const int lane = threadIdx.x & 31;
+        const unsigned long long up = __shfl_up_sync(kFull, k, 1);
+        const int g = base + lane;
+        k = g > pos ? (lane == 0 ? carry : up) : (g == pos ? c : k);
+    }
+    // knn_offer over the slots up to `last`: the position is the number of smaller keys in all of them, and the shift
+    // carries lane 31 of each slot into lane 0 of the next.
+    __device__ __forceinline__ void offer(unsigned long long cand) {
+        unsigned long long kth = kth_key();
+        unsigned pend = __ballot_sync(kFull, cand < kth);
+        while (pend) {
+            const int src = __ffs(pend) - 1;
+            pend &= pend - 1;
+            const unsigned long long c = __shfl_sync(kFull, cand, src);
+            if (c < kth) {
+                int pos = __popc(__ballot_sync(kFull, k0 < c));
+                if (last >= 1) pos += __popc(__ballot_sync(kFull, k1 < c));
+                if (last >= 2) pos += __popc(__ballot_sync(kFull, k2 < c));
+                if (last >= 3) pos += __popc(__ballot_sync(kFull, k3 < c));
+                if (last >= 3) shift(k3, 96, __shfl_sync(kFull, k2, 31), c, pos);
+                if (last >= 2) shift(k2, 64, __shfl_sync(kFull, k1, 31), c, pos);
+                if (last >= 1) shift(k1, 32, __shfl_sync(kFull, k0, 31), c, pos);
+                shift(k0, 0, 0ull, c, pos);
+                kth = kth_key();
+            }
+        }
+    }
+};
+
 // The sorted points [s, e), 32 at a time.
+template <typename List>
 __device__ __forceinline__ void knn_scan(const float4* __restrict__ pts, unsigned s, unsigned e, const KnnQuery& q,
-                                         unsigned long long& key, int kp) {
+                                         List& list) {
     const unsigned lane = threadIdx.x & 31;
     for (unsigned b = s; b < e; b += 32) {
         unsigned long long cand = ~0ull;
         if (b + lane < e) {
             const float4 t = __ldg(&pts[b + lane]);
             const float d = dist2_canonical(t, q.x, q.y, q.z);
-            cand = ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)__float_as_int(t.w);
+            if (list.accept(d)) cand = ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)__float_as_int(t.w);
         }
-        knn_offer(key, kp, cand);
+        list.offer(cand);
     }
 }
 
 // Every cell of box b that is not in box `skip`, one (grid-y, grid-z) row per lane: a row's cells are one contiguous
 // run of pts4 (two when `skip` cuts it).  A row whose lower bound exceeds the k-th distance is not read.
+template <typename List>
 __device__ __forceinline__ void knn_visit_box(const KnnView& v, const KnnQuery& q, const CellBox& b, const CellBox& skip,
-                                           unsigned long long& key, int kp) {
+                                              List& list) {
     const Grid& g = v.g;
     const int lane = threadIdx.x & 31;
     const int wy = b.y1 - b.y0 + 1;
     const int rows = wy * (b.z1 - b.z0 + 1);
     const float ex = axis_gap(q.gx, g.ox, g.cx, b.x0, b.x1, q.sx);
     for (int base = 0; base < rows; base += 32) {
-        const float kth = kth_dist2(key, kp);
+        const float kth = list.bound();
         unsigned s1 = 0, e1 = 0, s2 = 0, e2 = 0;
         float lb = 0.f;
         if (base + lane < rows) {
@@ -235,9 +295,9 @@ __device__ __forceinline__ void knn_visit_box(const KnnView& v, const KnnQuery& 
             const int src = __ffs(todo) - 1;
             todo &= todo - 1;
             const float rlb = __shfl_sync(kFull, lb, src);
-            if (kth_dist2(key, kp) < rlb) continue;   // the list tightened since the row was tested
-            knn_scan(v.pts, __shfl_sync(kFull, s1, src), __shfl_sync(kFull, e1, src), q, key, kp);
-            knn_scan(v.pts, __shfl_sync(kFull, s2, src), __shfl_sync(kFull, e2, src), q, key, kp);
+            if (list.bound() < rlb) continue;   // the list tightened since the row was tested
+            knn_scan(v.pts, __shfl_sync(kFull, s1, src), __shfl_sync(kFull, e1, src), q, list);
+            knn_scan(v.pts, __shfl_sync(kFull, s2, src), __shfl_sync(kFull, e2, src), q, list);
         }
     }
 }
@@ -249,7 +309,8 @@ __device__ __forceinline__ void knn_visit_box(const KnnView& v, const KnnQuery& 
 //      round visits the non-empty blocks of its shell whose lower bound does not exceed the k-th distance, and the
 //      search ends after the first round whose box bounds every point outside it beyond the k-th distance, or
 //      which covers the grid.  Empty blocks cost one flag load, 32 per warp step.
-__device__ __forceinline__ void knn_query(const KnnView& v, const KnnQuery& q, int kp, unsigned long long& key) {
+template <typename List>
+__device__ __forceinline__ void knn_query(const KnnView& v, const KnnQuery& q, List& list) {
     const Grid& g = v.g;
     const int lane = threadIdx.x & 31;
     const int cx = cell1(q.gx, g.ox, g.inv_cx, g.nx), cy = cell1(q.gy, g.oy, g.inv_c, g.ny),
@@ -257,8 +318,8 @@ __device__ __forceinline__ void knn_query(const KnnView& v, const KnnQuery& q, i
     const CellBox near{max(cx - 1, 0), min(cx + 1, g.nx - 1), max(cy - 1, 0),
                        min(cy + 1, g.ny - 1), max(cz - 1, 0), min(cz + 1, g.nz - 1)};
     const CellBox none{0, -1, 0, -1, 0, -1};
-    knn_visit_box(v, q, near, none, key, kp);
-    if (kth_dist2(key, kp) < box_clearance2(g, q, near)) return;
+    knn_visit_box(v, q, near, none, list);
+    if (list.bound() < box_clearance2(g, q, near)) return;
 
     const int bx = cx >> kBlockShift, by = cy >> kBlockShift, bz = cz >> kBlockShift;
     int done = -1;   // blocks within this Chebyshev radius are visited
@@ -288,18 +349,18 @@ __device__ __forceinline__ void knn_query(const KnnView& v, const KnnQuery& q, i
                     visit = true;
                 }
             }
-            const float kth = kth_dist2(key, kp);   // every lane shuffles: not inside the short-circuit below
+            const float kth = list.bound();   // every lane shuffles: not inside the short-circuit below
             unsigned todo = __ballot_sync(kFull, visit && !(kth < lb));
             while (todo) {
                 const int src = __ffs(todo) - 1;
                 todo &= todo - 1;
-                if (kth_dist2(key, kp) < __shfl_sync(kFull, lb, src)) continue;
+                if (list.bound() < __shfl_sync(kFull, lb, src)) continue;
                 const int px = __shfl_sync(kFull, ix, src), py = __shfl_sync(kFull, iy, src),
                           pz = __shfl_sync(kFull, iz, src);
                 const CellBox blk{px << kBlockShift, min(((px + 1) << kBlockShift) - 1, g.nx - 1),
                                   py << kBlockShift, min(((py + 1) << kBlockShift) - 1, g.ny - 1),
                                   pz << kBlockShift, min(((pz + 1) << kBlockShift) - 1, g.nz - 1)};
-                knn_visit_box(v, q, blk, near, key, kp);
+                knn_visit_box(v, q, blk, near, list);
             }
         }
         done = r;
@@ -307,9 +368,17 @@ __device__ __forceinline__ void knn_query(const KnnView& v, const KnnQuery& q, i
                            y0 << kBlockShift, min(((y1 + 1) << kBlockShift) - 1, g.ny - 1),
                            z0 << kBlockShift, min(((z1 + 1) << kBlockShift) - 1, g.nz - 1)};
         if ((x0 == 0 && y0 == 0 && z0 == 0 && x1 == v.nbx - 1 && y1 == v.nby - 1 && z1 == v.nbz - 1) ||
-            kth_dist2(key, kp) < box_clearance2(g, q, seen))
+            list.bound() < box_clearance2(g, q, seen))
             return;
     }
+}
+
+// The grid coordinates and slacks of a query whose real coordinates are set.
+__device__ __forceinline__ void knn_query_setup(const Grid& g, KnnQuery& q) {
+    to_grid(g, q.x, q.y, q.z, q.gx, q.gy, q.gz);
+    q.sx = g.tol + fabsf(q.gx) * 2.4e-7f;
+    q.sy = g.tol + fabsf(q.gy) * 2.4e-7f;
+    q.sz = g.tol + fabsf(q.gz) * 2.4e-7f;
 }
 
 // One warp per query: lane j writes the j-th neighbour.  A query with a non-finite coordinate gets -1 / 0.
@@ -325,19 +394,57 @@ __global__ void knn_search_kernel(KnnView v, const float* __restrict__ queries, 
     q.x = queries[3 * qi];
     q.y = queries[3 * qi + 1];
     q.z = queries[3 * qi + 2];
-    unsigned long long key = ~0ull;
+    KnnList list;
+    list.kp = kp;
     if (isfinite(q.x) && isfinite(q.y) && isfinite(q.z)) {
-        to_grid(v.g, q.x, q.y, q.z, q.gx, q.gy, q.gz);
-        q.sx = v.g.tol + fabsf(q.gx) * 2.4e-7f;
-        q.sy = v.g.tol + fabsf(q.gy) * 2.4e-7f;
-        q.sz = v.g.tol + fabsf(q.gz) * 2.4e-7f;
-        knn_query(v, q, kp, key);
+        knn_query_setup(v.g, q);
+        knn_query(v, q, list);
     }
+    const unsigned long long key = list.key;
     if (lane < kp) {
         const bool ok = key != ~0ull;
         if (idx) idx[qi * kp + lane] = ok ? (IndexT)(int)(unsigned)key : (IndexT)-1;
         if (d2) d2[qi * kp + lane] = ok ? __uint_as_float((unsigned)(key >> 32)) : 0.f;
     }
+}
+
+// One warp per query, up to four keys per lane: the kp nearest points with dist^2 <= thr (+inf: no cap),
+// ascending by (dist^2, index).  Slot g = 32 s + lane of row qi gets the g-th neighbour, -1 / 0 past cnt[qi].  With
+// thr = +inf this is knn_search_kernel's list; with thr = (float)r * (float)r and kp <= 32 it is the hybrid search's,
+// whose distance is the same dist2_canonical and whose order is the same key.  Queries are finite (the callers
+// check; a guard here costs the kernel its fit in 80 registers).
+__global__ void __launch_bounds__(kThreads) knn_lists_kernel(KnnView v, const float* __restrict__ queries, int64_t nq,
+                                                             int kp, float thr, int32_t* __restrict__ idx,
+                                                             float* __restrict__ d2, int32_t* __restrict__ cnt) {
+    const int64_t qi = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (qi >= nq) return;
+    KnnQuery q;
+    q.x = queries[3 * qi];
+    q.y = queries[3 * qi + 1];
+    q.z = queries[3 * qi + 2];
+    knn_query_setup(v.g, q);
+    KnnWideList list(kp, thr);
+    knn_query(v, q, list);
+    const unsigned long long keys[4] = {list.k0, list.k1, list.k2, list.k3};
+    int c = 0;
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+        const int g = 32 * s + lane;
+        const bool ok = g < kp && keys[s] != ~0ull;
+        c += __popc(__ballot_sync(kFull, ok));
+        if (g < kp) {
+            idx[qi * kp + g] = ok ? (int32_t)(unsigned)keys[s] : -1;
+            d2[qi * kp + g] = ok ? __uint_as_float((unsigned)(keys[s] >> 32)) : 0.f;
+        }
+    }
+    if (lane == 0) cnt[qi] = c;
+}
+
+// *bad = 1 when a query coordinate is NaN or infinite
+__global__ void knn_finite_kernel(const float* __restrict__ q, int64_t n, unsigned* __restrict__ bad) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i < n) flag_nonfinite(q, i, bad);
 }
 
 // ------------------------------------------------------------------ deterministic sums
@@ -450,6 +557,18 @@ static int knn_dist2(const float* data, int64_t m, const float* queries, int64_t
     return o3db_knn_search(index.get(), queries, nq, k, O3DB_INDEX_INT32, nullptr, d2.get(), st);
 }
 
+int knn_lists(const o3db_knn* knn, const float* queries, int64_t nq, int k, float thr, int32_t* idx, float* d2,
+              int32_t* cnt, cudaStream_t st) {
+    O3DB_REQUIRE(knn != nullptr, "knn_lists: null index");
+    O3DB_REQUIRE(k >= 1 && k <= kKnnWideMax, "knn_lists: k = %d is not in 1..%d", k, kKnnWideMax);
+    if (nq == 0) return O3DB_OK;
+    const int kp = (int)std::min<int64_t>(k, knn->grid.m);
+    knn_lists_kernel<<<(unsigned)ceil_div(nq, kThreads / 32), kThreads, 0, st>>>(
+            knn_view(knn), queries, nq, kp, thr, idx, d2, cnt);
+    O3DB_LAUNCH_CHECK();
+    return O3DB_OK;
+}
+
 // Sum of the per-block partials, in block order, after a synchronise.
 template <typename T>
 static int read_partials(const T* dev, size_t count, std::vector<T>& host, cudaStream_t st) {
@@ -551,6 +670,29 @@ int o3db_knn_search(const o3db_knn* knn, const float* queries_dev, int64_t num_q
                                                             static_cast<int64_t*>(indices_dev), distances_dev);
     O3DB_LAUNCH_CHECK();
     return O3DB_OK;
+}
+
+int o3db_knn_search_lists(const o3db_knn* knn, const float* queries_dev, int64_t num_queries, int knn_k, double radius,
+                          int32_t* indices_dev, float* distances_dev, int32_t* counts_dev, void* stream) {
+    O3DB_REQUIRE(knn != nullptr, "Index is not set.");
+    O3DB_REQUIRE(knn_k >= 1 && knn_k <= kKnnWideMax, "knn = %d is not in 1..%d", knn_k, kKnnWideMax);
+    O3DB_REQUIRE(radius >= 0 && std::isfinite(radius), "o3db_knn_search_lists: radius must be finite and >= 0 (got %g)",
+                 radius);
+    O3DB_REQUIRE(num_queries >= 0, "o3db_knn_search_lists: negative query count");
+    if (num_queries == 0) return O3DB_OK;
+    O3DB_REQUIRE(queries_dev && indices_dev && distances_dev && counts_dev, "o3db_knn_search_lists: null argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    DevPtr<unsigned> bad;
+    if (int rc = dev_alloc(bad, 1, st)) return rc;
+    O3DB_CUDA_CHECK(cudaMemsetAsync(bad.get(), 0, sizeof(unsigned), st));
+    knn_finite_kernel<<<(unsigned)ceil_div(num_queries, kThreads), kThreads, 0, st>>>(queries_dev, num_queries, bad.get());
+    O3DB_LAUNCH_CHECK();
+    unsigned h_bad = 0;
+    O3DB_CUDA_CHECK(cudaMemcpyAsync(&h_bad, bad.get(), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    O3DB_CUDA_CHECK(cudaStreamSynchronize(st));
+    O3DB_REQUIRE(h_bad == 0, "o3db_knn_search_lists: the queries have non-finite coordinates");
+    const float thr = radius > 0 ? (float)radius * (float)radius : INFINITY;
+    return knn_lists(knn, queries_dev, num_queries, knn_k, thr, indices_dev, distances_dev, counts_dev, st);
 }
 
 int o3db_remove_statistical_outliers(const float* positions_dev, int64_t n, int nb_neighbors, double std_ratio,

@@ -10,6 +10,7 @@ results into the reference's result type.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass, field
 from enum import IntEnum
 
@@ -453,6 +454,82 @@ def evaluate_registration(source, target, max_correspondence_distance, transform
     res, _, _ = _run_single_scale(source, target, max_correspondence_distance, T, est, crit, None, 0, 0)
     res.transformation = T.copy()
     return res
+
+
+def compute_fpfh_feature(input, max_nn=100, radius=None, indices=None):
+    """ComputeFPFHFeature (t/pipelines/registration/Feature.cpp:23-277; pybind feature.cpp) -> torch.float32 [rows, 33]
+    on the cloud's device.  With max_nn and radius (the recommended hybrid call) each point's neighbours are the
+    max_nn nearest within radius; with radius=None the min(max_nn, n) nearest.  max_nn must be in 4..128; radius-only
+    mode (max_nn=None) raises, because the fixed-radius search is not built.  indices (any int sequence or tensor)
+    selects rows: one per distinct index, in ascending point order, each equal to that point's row without indices.
+    f64 clouds, non-finite positions and non-finite normal components raise (DESIGN.md §4.24, §7)."""
+    if max_nn is not None and int(max_nn) <= 3:
+        raise RuntimeError("max_nn must be greater than 3.")
+    if radius is not None and not float(radius) > 0:
+        raise RuntimeError("radius must be greater than 0.")
+    if radius is not None and not math.isfinite(float(radius)):
+        raise RuntimeError(f"ComputeFPFHFeature: radius must be finite (got {float(radius)})")
+    p = input._positions_f32("ComputeFPFHFeature")
+    n = int(p.shape[0])
+    # an empty cloud has no normal rows to check: it gives [0, 33] (DESIGN.md §7)
+    if n > 0 and not input.has_point_normals():
+        raise RuntimeError("The input point cloud has no normal.")
+    if max_nn is None and radius is None:
+        raise RuntimeError("Both max_nn and radius are none.")
+    if max_nn is None:
+        raise RuntimeError("ComputeFPFHFeature: radius-only search is not supported by open3d_b200; use the hybrid "
+                           "call compute_fpfh_feature(input, max_nn=100, radius=radius)")
+    max_nn = int(max_nn)
+    if max_nn > 128:
+        raise RuntimeError(f"ComputeFPFHFeature: max_nn = {max_nn} exceeds the largest list this search supports (128)")
+    if n == 0:
+        return torch.zeros((0, 33), dtype=torch.float32, device=p.device)
+    nrm = input._normals_f32(n)
+    sel = None
+    if indices is not None:
+        sel = torch.as_tensor(indices, device=p.device).reshape(-1)
+        if sel.numel() == 0:   # an empty sequence has no dtype of its own
+            return torch.zeros((0, 33), dtype=torch.float32, device=p.device)
+        if sel.dtype.is_floating_point or sel.dtype.is_complex or sel.dtype == torch.bool:
+            raise RuntimeError(f"ComputeFPFHFeature: indices must be integers (got {sel.dtype})")
+        sel = sel.to(torch.int64).contiguous()
+    rows = n if sel is None else min(n, int(sel.numel()))
+    out = torch.zeros((rows, 33), dtype=torch.float32, device=p.device)
+    got = C.c_int64(0)
+    check(lib.o3db_compute_fpfh_feature(p.data_ptr(), nrm.data_ptr(), n, max_nn,
+                                        0.0 if radius is None else float(radius),
+                                        None if sel is None else sel.data_ptr(), -1 if sel is None else int(sel.numel()),
+                                        out.data_ptr() if rows else None, C.byref(got), current_stream_ptr()))
+    return out[:got.value]
+
+
+def correspondences_from_features(source_features, target_features, mutual_filter=False,
+                                  mutual_consistency_ratio=0.1):
+    """CorrespondencesFromFeatures (t/pipelines/registration/Feature.cpp:279-333) -> torch.int64 [K, 2] on the device:
+    (source row, nearest target row) by the f32 squared feature distance, ties to the lowest target index.  With
+    mutual_filter only the mutual pairs are kept, when there are more than mutual_consistency_ratio * N of them; else
+    every pair, with upstream's warning.  Features are [N, D] and [M, D] Float32 with the same D >= 1."""
+    def _rows(x, name):
+        x = torch.as_tensor(x)
+        if x.dtype != torch.float32 or x.dim() != 2 or x.shape[1] < 1:
+            raise RuntimeError(f"{name} must be a [N, D] Float32 tensor with D >= 1 (got {tuple(x.shape)} {x.dtype})")
+        if not x.is_cuda and torch.cuda.is_available():
+            x = x.cuda()
+        return x.contiguous()
+    s, t = _rows(source_features, "source_features"), _rows(target_features, "target_features")
+    if s.shape[1] != t.shape[1]:
+        raise RuntimeError(f"source and target features have different dimensions ({s.shape[1]} and {t.shape[1]})")
+    n = int(s.shape[0])
+    out = torch.empty((n, 2), dtype=torch.int64, device=s.device)
+    k, mutual = C.c_int64(0), C.c_int64(0)
+    ratio = float(np.float32(mutual_consistency_ratio))
+    check(lib.o3db_correspondences_from_features(s.data_ptr(), n, t.data_ptr(), int(t.shape[0]), int(s.shape[1]),
+                                                 int(bool(mutual_filter)), ratio, out.data_ptr() if n else None,
+                                                 C.byref(k), C.byref(mutual), current_stream_ptr()))
+    if mutual_filter and n and k.value == n and not np.float32(mutual.value) > np.float32(ratio) * np.float32(n):
+        print(f"[Open3D WARNING] Too few correspondences ({mutual.value:d}) after mutual filter, fall back to "
+              "original correspondences.")
+    return out[:k.value]
 
 
 def get_information_matrix(source, target, max_correspondence_distance, transformation):
