@@ -231,6 +231,57 @@ int o3db_farthest_point_down_sample(const float* positions_dev /* [n,3] */, int6
  * index from std::uniform_int_distribution<size_t>(0, n-1), a repeat within a row redrawn.  Host only. */
 int o3db_random_seed(int seed);
 int o3db_random_sample_indices(int64_t n, int sample_size, int num_samples, int64_t* out_host);
+/* count draws of upstream's UniformIntGenerator<int>(low, high) (utility/Random.h:63-90): each one
+ * std::uniform_int_distribution<int>(low, high) from the engine, with replacement; upstream's messages for low < 0 and
+ * low > high.  Host only. */
+int o3db_random_uniform_ints(int low, int high, int64_t count, int* out_host);
+
+/* ------------------------------------------------------------------------
+ * Global registration by RANSAC — pipelines::registration::RegistrationRANSACBasedOnCorrespondence
+ * (pipelines/registration/Registration.cpp:195-379) with TransformationEstimationPointToPoint(false) and the checkers
+ * of CorrespondenceChecker.cpp, on Float32 clouds.  The result is that of upstream's function run on one thread
+ * (DESIGN.md §4.25):
+ *   draws       hypothesis i takes ransac_n draws of std::uniform_int_distribution<int>(0, K-1) from the library's
+ *               engine, in order, and is drawn only while i < est_k; afterwards the engine has advanced by exactly
+ *               stop * ransac_n draws, stop the first i not below est_k;
+ *   hypothesis  f64: means as the sums in sample order times 1/ransac_n, the cross-covariance of the demeaned pairs
+ *               times 1/ransac_n, the library's Jacobi Kabsch rotation, t = mean_t - R mean_s; every op rounded, no FMA;
+ *   checkers    edge length (similarity), distance (threshold) and normal (the cosine of the angle, computed by the
+ *               caller with std::cos); the normal checker passes where either normal pointer is null;
+ *   validation  the source transformed in f64, ((T_j0 x + T_j1 y) + T_j2 z) + T_j3; its nearest target point by
+ *               ((dx^2 + dy^2) + dz^2) in f64, a match when d^2 < max_correspondence_distance^2, ties to the lowest
+ *               index; fitness = matches / n, rmse = sqrt(sum d^2 / matches), the sum over tiles of 128 points in
+ *               index order, then over the tiles;
+ *   selection   upstream's IsBetterRANSACThan and est_k rule from the inlier ratio of all K pairs.
+ * transformation_host [16] receives the best transformation, row-major (the identity when nothing won);
+ * correspondence_set_dev [n] the best transformation's nearest target point of each source point, -1 for none.
+ * Nothing is drawn and the result is the identity with no correspondences when ransac_n < 3, K < ransac_n,
+ * max_correspondence_distance <= 0 or max_iteration <= 0.  Errors: a non-finite distance, non-finite positions (the
+ * message names remove_non_finite_points), a pair outside [0, n) x [0, m), counts of 2^31 - 1 or more, null pointers.
+ * The call synchronises the stream 2 + 2 * batches times, a batch being 8192 hypotheses (fewer for ransac_n > 512): the
+ * index build, each batch's passing count and end state, and the result. */
+typedef struct {
+    int use_edge_length, use_distance, use_normal;
+    double edge_length_similarity;
+    double distance_threshold;
+    double cos_normal_angle_threshold;
+} o3db_ransac_checkers;
+
+typedef struct {
+    int64_t drawn;        /* hypotheses drawn: stop */
+    int64_t validated;    /* hypotheses that passed the checkers before stop */
+    int64_t best_index;   /* draw index of the best hypothesis, -1 for none */
+    double fitness;
+    double inlier_rmse;
+} o3db_ransac_stats;
+
+int o3db_registration_ransac(const float* source_dev /* [n,3] */, const float* source_normals_dev /* or NULL */,
+                             int64_t n, const float* target_dev /* [m,3] */,
+                             const float* target_normals_dev /* or NULL */, int64_t m,
+                             const int64_t* correspondences_dev /* [K,2] */, int64_t K,
+                             double max_correspondence_distance, int ransac_n, int max_iteration, double confidence,
+                             const o3db_ransac_checkers* checkers /* or NULL */, double* transformation_host /* [16] */,
+                             int64_t* correspondence_set_dev /* [n] */, o3db_ransac_stats* stats, void* stream);
 
 /* ------------------------------------------------------------------------
  * RANSAC plane segmentation — geometry::PointCloud::SegmentPlane (geometry/PointCloudSegmentation.cpp:157-279), which

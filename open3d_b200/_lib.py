@@ -57,6 +57,17 @@ class SegmentStats(C.Structure):
                 ("inlier_rmse", C.c_double)]
 
 
+class RansacCheckers(C.Structure):
+    _fields_ = [("use_edge_length", C.c_int), ("use_distance", C.c_int), ("use_normal", C.c_int),
+                ("edge_length_similarity", C.c_double), ("distance_threshold", C.c_double),
+                ("cos_normal_angle_threshold", C.c_double)]
+
+
+class RansacStats(C.Structure):
+    _fields_ = [("drawn", C.c_int64), ("validated", C.c_int64), ("best_index", C.c_int64), ("fitness", C.c_double),
+                ("inlier_rmse", C.c_double)]
+
+
 class RaycastOutputs(C.Structure):
     """o3db_raycast_outputs: device pointers, None = attribute not requested"""
     _fields_ = [(n, C.c_void_p) for n in ("depth", "vertex", "color", "normal", "index", "mask", "interp_ratio",
@@ -91,6 +102,9 @@ _SIGS = {
     "o3db_farthest_point_down_sample": (_i, [_vp, _i64, _i64, _i64, _vp, _vp]),
     "o3db_random_seed": (_i, [_i]),
     "o3db_random_sample_indices": (_i, [_i64, _i, _i, _vp]),
+    "o3db_random_uniform_ints": (_i, [_i, _i, _i64, _vp]),
+    "o3db_registration_ransac": (_i, [_vp, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _dbl, _i, _i, _dbl,
+                                      C.POINTER(RansacCheckers), _dp, _vp, C.POINTER(RansacStats), _vp]),
     "o3db_segment_plane": (_i, [_vp, _i64, _dbl, _i, _i, _dbl, _vp, _vp, C.POINTER(_i64), C.POINTER(SegmentStats),
                                 _vp]),
     "o3db_compute_pose_point_to_plane": (_i, [_vp, _vp, _vp, _vp, _i64, C.POINTER(RobustKernel), _vp, _vp,

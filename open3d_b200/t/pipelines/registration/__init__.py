@@ -532,6 +532,155 @@ def correspondences_from_features(source_features, target_features, mutual_filte
     return out[:k.value]
 
 
+class RANSACConvergenceCriteria:
+    """RANSACConvergenceCriteria (pipelines/registration/Registration.h:54-76; pybind registration.cpp:877-905):
+    max_iteration hypotheses at most, and the confidence that sets the early stop, clamped to [0, 1] (a NaN stays
+    NaN, as std::max(std::min(c, 1.0), 0.0) leaves it)."""
+
+    def __init__(self, max_iteration=100000, confidence=0.999):
+        self.max_iteration = int(max_iteration)
+        c = float(confidence)
+        self.confidence = c if math.isnan(c) else max(min(c, 1.0), 0.0)
+
+    def __repr__(self):
+        return (f"RANSACConvergenceCriteria[max_iteration_={self.max_iteration:d}, "
+                f"confidence_={self.confidence:e}].")
+
+
+class CorrespondenceChecker:
+    """CorrespondenceChecker (pipelines/registration/CorrespondenceChecker.h:28-63): the checkers RANSAC runs on each
+    sample before validating it.  Only the three subclasses below run on the device."""
+    require_pointcloud_alignment = False
+
+
+class CorrespondenceCheckerBasedOnEdgeLength(CorrespondenceChecker):
+    """Rejects a sample when an edge between two of its source points and the matching target edge differ by more than
+    the similarity ratio (CorrespondenceChecker.cpp:19-40)."""
+
+    def __init__(self, similarity_threshold=0.9):
+        self.similarity_threshold = float(similarity_threshold)
+
+
+class CorrespondenceCheckerBasedOnDistance(CorrespondenceChecker):
+    """Rejects a sample when a transformed source point lies farther than distance_threshold from its target
+    point (CorrespondenceChecker.cpp:42-57)."""
+    require_pointcloud_alignment = True
+
+    def __init__(self, distance_threshold):
+        self.distance_threshold = float(distance_threshold)
+
+
+class CorrespondenceCheckerBasedOnNormal(CorrespondenceChecker):
+    """Rejects a sample when a rotated source normal and its target normal are more than normal_angle_threshold
+    (radians) apart (CorrespondenceChecker.cpp:59-80).  Passes, with upstream's warning, when a cloud has no
+    normals."""
+    require_pointcloud_alignment = True
+
+    def __init__(self, normal_angle_threshold):
+        self.normal_angle_threshold = float(normal_angle_threshold)
+
+
+def _ransac_checkers(checkers):
+    """The C checker struct.  Several checkers of one kind reject what any of them rejects: the smallest distance, the
+    largest similarity and the largest cosine, leaving out NaN thresholds, which reject nothing."""
+    from ...._lib import RansacCheckers
+    edge, dist, cosn = [], [], []
+    for c in checkers or ():
+        if type(c) is CorrespondenceCheckerBasedOnEdgeLength:
+            edge.append(c.similarity_threshold)
+        elif type(c) is CorrespondenceCheckerBasedOnDistance:
+            dist.append(c.distance_threshold)
+        elif type(c) is CorrespondenceCheckerBasedOnNormal:
+            cosn.append(math.cos(c.normal_angle_threshold))
+        else:
+            raise RuntimeError(f"RegistrationRANSAC: unsupported checker {type(c).__name__}; the supported ones are "
+                               "CorrespondenceCheckerBasedOnEdgeLength, CorrespondenceCheckerBasedOnDistance and "
+                               "CorrespondenceCheckerBasedOnNormal")
+
+    def pick(vals, f):
+        finite = [v for v in vals if not math.isnan(v)]
+        return f(finite) if finite else math.nan
+    return RansacCheckers(int(bool(edge)), int(bool(dist)), int(bool(cosn)), pick(edge, max), pick(dist, min),
+                          pick(cosn, max))
+
+
+def _ransac_correspondences(corres, device):
+    c = torch.as_tensor(corres)
+    if c.dtype not in (torch.int32, torch.int64) or c.dim() != 2 or c.shape[1] != 2:
+        raise RuntimeError(f"RegistrationRANSAC: corres must be an Int32 or Int64 [K, 2] tensor (got "
+                           f"{tuple(c.shape)} {c.dtype})")
+    return c.to(device=device, dtype=torch.int64).contiguous()
+
+
+def _registration_ransac(source, target, corres, max_correspondence_distance, estimation_method, ransac_n, checkers,
+                         criteria):
+    """o3db_registration_ransac -> (RegistrationResult, RansacStats)."""
+    from ...._lib import RansacStats
+    if estimation_method is not None and (type(estimation_method) is not TransformationEstimationPointToPoint or
+                                           getattr(estimation_method, "with_scaling", False)):
+        raise RuntimeError("RegistrationRANSAC: only TransformationEstimationPointToPoint() without scaling is "
+                           f"supported (got {type(estimation_method).__name__})")
+    criteria = RANSACConvergenceCriteria() if criteria is None else criteria
+    ransac_n, max_iteration = int(ransac_n), int(criteria.max_iteration)
+    for name, v in (("ransac_n", ransac_n), ("max_iteration", max_iteration)):
+        if not -2 ** 31 <= v < 2 ** 31:
+            raise TypeError(f"RegistrationRANSAC: {name} must fit in a 32-bit int (got {v})")
+    chk = _ransac_checkers(checkers)
+    s = source._positions_f32("RegistrationRANSAC")
+    t = target._positions_f32("RegistrationRANSAC")
+    n, m = int(s.shape[0]), int(t.shape[0])
+    c = _ransac_correspondences(corres, s.device)
+    sn = source._normals_f32(n) if source.has_point_normals() else None
+    tn = target._normals_f32(m) if target.has_point_normals() else None
+    if chk.use_normal and (sn is None or tn is None) and ransac_n >= 3 and c.shape[0] >= ransac_n and \
+            max_correspondence_distance > 0 and max_iteration > 0:
+        print("[Open3D WARNING] [CorrespondenceCheckerBasedOnNormal::Check] Pointcloud has no normals.")
+    T = np.zeros(16, np.float64)
+    out = torch.empty((n,), dtype=torch.int64, device=s.device)
+    stats = RansacStats()
+    check(lib.o3db_registration_ransac(s.data_ptr(), None if sn is None else sn.data_ptr(), n, t.data_ptr(),
+                                       None if tn is None else tn.data_ptr(), m, c.data_ptr(), int(c.shape[0]),
+                                       float(max_correspondence_distance), ransac_n, max_iteration,
+                                       float(criteria.confidence), C.byref(chk), dptr(T),
+                                       out.data_ptr() if n else None, C.byref(stats), current_stream_ptr()))
+    res = RegistrationResult(T.reshape(4, 4), out, stats.inlier_rmse, stats.fitness)
+    return res, stats
+
+
+def registration_ransac_based_on_correspondence(source, target, corres, max_correspondence_distance,
+                                                estimation_method=None, ransac_n=3, checkers=None, criteria=None):
+    """RegistrationRANSACBasedOnCorrespondence (pipelines/registration/Registration.cpp:343-379; pybind
+    registration.cpp), run as upstream runs it on one thread, on the device (o3db_registration_ransac).  corres is an
+    Int32 or Int64 [K, 2] tensor or array of (source row, target row), as correspondences_from_features returns.
+    Hypotheses draw from the library's random engine (open3d_b200.utility.random.seed).  estimation_method is None or
+    TransformationEstimationPointToPoint(); checkers any of the three CorrespondenceChecker subclasses.  The result's
+    transformation is 4x4 Float64 numpy; correspondence_set is Int64 [n] on the device, -1 for no match (upstream's
+    pair list is its (nonzero, value)); converged and num_iterations are False and 0.  Float64 clouds, non-finite
+    positions, a non-finite distance and pairs outside the clouds raise (DESIGN.md §4.25, §7)."""
+    return _registration_ransac(source, target, corres, max_correspondence_distance, estimation_method, ransac_n,
+                                checkers, criteria)[0]
+
+
+def registration_ransac_based_on_feature_matching(source, target, source_feature, target_feature, mutual_filter,
+                                                  max_correspondence_distance, estimation_method=None, ransac_n=3,
+                                                  checkers=None, criteria=None):
+    """RegistrationRANSACBasedOnFeatureMatching (pipelines/registration/Registration.cpp:381-404): the identity for
+    ransac_n < 3 or max_correspondence_distance <= 0, else correspondences_from_features(source_feature,
+    target_feature, mutual_filter) and registration_ransac_based_on_correspondence.  Features are [N, D] Float32,
+    as compute_fpfh_feature returns them, with one row per point of their cloud."""
+    if int(ransac_n) < 3 or max_correspondence_distance <= 0.0:
+        s = source._positions_f32("RegistrationRANSAC")
+        return RegistrationResult(np.eye(4), torch.full((int(s.shape[0]),), -1, dtype=torch.int64, device=s.device))
+    for f, cloud, name in ((source_feature, source, "source"), (target_feature, target, "target")):
+        rows = int(torch.as_tensor(f).shape[0])
+        npts = int(cloud._positions_f32("RegistrationRANSAC").shape[0])
+        if rows != npts:
+            raise RuntimeError(f"RegistrationRANSAC: the {name} feature has {rows} rows for {npts} points")
+    corres = correspondences_from_features(source_feature, target_feature, mutual_filter)
+    return registration_ransac_based_on_correspondence(source, target, corres, max_correspondence_distance,
+                                                       estimation_method, ransac_n, checkers, criteria)
+
+
 def get_information_matrix(source, target, max_correspondence_distance, transformation):
     """GetInformationMatrix (Registration.cpp:446-485; pybind registration.get_information_matrix): 6x6 Float64 GTG
     of the target points matched by the transformed source, on the host like upstream."""
