@@ -284,6 +284,60 @@ int o3db_registration_ransac(const float* source_dev /* [n,3] */, const float* s
                              int64_t* correspondence_set_dev /* [n] */, o3db_ransac_stats* stats, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Fast Global Registration — pipelines::registration::FastGlobalRegistrationBasedOnCorrespondence and
+ * FastGlobalRegistrationBasedOnFeatureMatching (pipelines/registration/FastGlobalRegistration.cpp:285-395, with
+ * NormalizePointCloud :143-195, AdvancedMatching :83-141, OptimizePairwiseRegistration :197-264,
+ * GetTransformationOriginalScale :268-282 and EvaluateRegistration, Registration.cpp:127-141), on Float32 clouds.
+ * The result is that of upstream's function run on one thread, in f64 with every op rounded and the Eigen orders of
+ * DESIGN.md §4.26:
+ *   pairs       correspondences_dev [K,2] (source row, target row); or, when it is NULL, the mutual nearest rows of
+ *               the [n,dim] and [m,dim] feature matrices (f32 squared distance, ties to the lowest row) in ascending
+ *               query row, the source's rows being the queries unless the tuple test runs and n < m;
+ *   normalise   each cloud's mean (the serial sum in point order / n), scale = the largest centred norm over both
+ *               clouds, scale_global = scale, or 1 with use_absolute_scale; "Invalid scale_global" when it is <= 0;
+ *   tuples      with tuple_test: nothing when there are at most 2 pairs (upstream's warning on stderr), else up to
+ *               100 x pairs trials of three std::uniform_int_distribution<int>(0, pairs-1) draws from the library's
+ *               engine, a trial passing when each of its three edges has li*tuple_scale < lj < li/tuple_scale, and the
+ *               loop stopping after the trial at which maximum_tuple_count tuples have passed; afterwards the engine
+ *               has advanced by exactly 3 x trials draws;
+ *   optimise    the identity for fewer than 10 pairs, else iteration_number Geman-McClure steps from par =
+ *               scale_global, with par /= division_factor every 4th step while decrease_mu and par >
+ *               maximum_correspondence_distance;
+ *   result      the inverse of the de-normalised transformation, evaluated on the original clouds: the nearest target
+ *               point of each transformed source point with d^2 < maximum_correspondence_distance^2, ties to the
+ *               lowest index; fitness = matches / n, rmse = sqrt(sum d^2 / matches), the sum over tiles of 128
+ *               points in index order, then over the tiles.
+ * transformation_host [16] receives the transformation, row-major; correspondence_set_dev [n] each source point's
+ * match, -1 for none.  Errors: a non-finite distance, non-finite positions, a pair outside [0, n) x [0, m), more than
+ * (2^31 - 1) / 100 pairs for the tuple test, counts of 2^31 - 1 or more, null pointers.  The call synchronises the
+ * stream 3 times, plus once per batch of 16384 tuple trials, plus twice in the feature matching. */
+typedef struct {
+    double division_factor;
+    int use_absolute_scale;
+    int decrease_mu;
+    double maximum_correspondence_distance;
+    int iteration_number;
+    double tuple_scale;
+    int maximum_tuple_count;
+    int tuple_test;
+} o3db_fgr_option;
+
+typedef struct {
+    int64_t cross;        /* the initial pairs: K, or the mutual feature matches */
+    int64_t tuples;       /* tuples that passed the tuple test */
+    int64_t trials;       /* tuple trials drawn: the engine advanced by 3 x trials */
+    int64_t pairs;        /* the pairs the optimisation ran on */
+    double fitness;
+    double inlier_rmse;
+} o3db_fgr_stats;
+
+int o3db_registration_fgr(const float* source_dev /* [n,3] */, int64_t n, const float* target_dev /* [m,3] */,
+                          int64_t m, const int64_t* correspondences_dev /* [K,2] or NULL */, int64_t K,
+                          const float* source_feature_dev /* [n,dim] */, const float* target_feature_dev /* [m,dim] */,
+                          int dim, const o3db_fgr_option* option, double* transformation_host /* [16] */,
+                          int64_t* correspondence_set_dev /* [n] */, o3db_fgr_stats* stats, void* stream);
+
+/* ------------------------------------------------------------------------
  * RANSAC plane segmentation — geometry::PointCloud::SegmentPlane (geometry/PointCloudSegmentation.cpp:157-279), which
  * t::geometry::PointCloud::SegmentPlane (t/geometry/PointCloud.cpp:1646-1666) runs on the host; Float32 positions.
  * The result is that of upstream's function run on one thread (DESIGN.md §4.21):

@@ -68,6 +68,17 @@ class RansacStats(C.Structure):
                 ("inlier_rmse", C.c_double)]
 
 
+class FgrOption(C.Structure):
+    _fields_ = [("division_factor", C.c_double), ("use_absolute_scale", C.c_int), ("decrease_mu", C.c_int),
+                ("maximum_correspondence_distance", C.c_double), ("iteration_number", C.c_int),
+                ("tuple_scale", C.c_double), ("maximum_tuple_count", C.c_int), ("tuple_test", C.c_int)]
+
+
+class FgrStats(C.Structure):
+    _fields_ = [("cross", C.c_int64), ("tuples", C.c_int64), ("trials", C.c_int64), ("pairs", C.c_int64),
+                ("fitness", C.c_double), ("inlier_rmse", C.c_double)]
+
+
 class RaycastOutputs(C.Structure):
     """o3db_raycast_outputs: device pointers, None = attribute not requested"""
     _fields_ = [(n, C.c_void_p) for n in ("depth", "vertex", "color", "normal", "index", "mask", "interp_ratio",
@@ -105,6 +116,8 @@ _SIGS = {
     "o3db_random_uniform_ints": (_i, [_i, _i, _i64, _vp]),
     "o3db_registration_ransac": (_i, [_vp, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _dbl, _i, _i, _dbl,
                                       C.POINTER(RansacCheckers), _dp, _vp, C.POINTER(RansacStats), _vp]),
+    "o3db_registration_fgr": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i, C.POINTER(FgrOption), _dp, _vp,
+                                   C.POINTER(FgrStats), _vp]),
     "o3db_segment_plane": (_i, [_vp, _i64, _dbl, _i, _i, _dbl, _vp, _vp, C.POINTER(_i64), C.POINTER(SegmentStats),
                                 _vp]),
     "o3db_compute_pose_point_to_plane": (_i, [_vp, _vp, _vp, _vp, _i64, C.POINTER(RobustKernel), _vp, _vp,

@@ -11,10 +11,11 @@ FLAGS=("${ARCH[@]}" -lineinfo -O3 -std=c++17
 cd "${HERE}"
 OBJS=()
 PIDS=()
-for f in common icp tsdf comm pointcloud raycast odometry extract projection knn smooth dbscan fps segment boundary remove fpfh ransac; do
+for f in common icp tsdf comm pointcloud raycast odometry extract projection knn smooth dbscan fps segment boundary remove fpfh ransac fgr; do
   EXTRA=()
-  # ransac.cu states one evaluation order for its f64 arithmetic: every op rounded, no FMA (DESIGN.md §4.25)
-  [[ "${f}" == ransac ]] && EXTRA=(-fmad=false)
+  # ransac.cu and fgr.cu state one evaluation order for their f64 arithmetic: every op rounded, no FMA
+  # (DESIGN.md §4.25, §4.26)
+  [[ "${f}" == ransac || "${f}" == fgr ]] && EXTRA=(-fmad=false)
   "${NVCC}" "${FLAGS[@]}" "${EXTRA[@]}" -c "${f}.cu" -o "${f}.o" &
   PIDS+=($!)
   OBJS+=("${f}.o")

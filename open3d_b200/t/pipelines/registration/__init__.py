@@ -681,6 +681,108 @@ def registration_ransac_based_on_feature_matching(source, target, source_feature
                                                        estimation_method, ransac_n, checkers, criteria)
 
 
+class FastGlobalRegistrationOption:
+    """FastGlobalRegistrationOption (pipelines/registration/FastGlobalRegistration.h:28-90) with the defaults of
+    upstream's Python binding (pybind registration.cpp), where decrease_mu is False."""
+
+    def __init__(self, division_factor=1.4, use_absolute_scale=False, decrease_mu=False,
+                 maximum_correspondence_distance=0.025, iteration_number=64, tuple_scale=0.95,
+                 maximum_tuple_count=1000, tuple_test=True):
+        self.division_factor = float(division_factor)
+        self.use_absolute_scale = bool(use_absolute_scale)
+        self.decrease_mu = bool(decrease_mu)
+        self.maximum_correspondence_distance = float(maximum_correspondence_distance)
+        self.iteration_number = int(iteration_number)
+        self.tuple_scale = float(tuple_scale)
+        self.maximum_tuple_count = int(maximum_tuple_count)
+        self.tuple_test = bool(tuple_test)
+
+    def __repr__(self):
+        def num(x):   # fmt's {} of a double: the shortest round trip, without a trailing ".0"
+            r = repr(float(x))
+            return r[:-2] if r.endswith(".0") else r
+
+        def b(x):
+            return "true" if x else "false"
+        return (f"FastGlobalRegistrationOption(\ndivision_factor={num(self.division_factor)},"
+                f"\nuse_absolute_scale={b(self.use_absolute_scale)},\ndecrease_mu={b(self.decrease_mu)},"
+                f"\nmaximum_correspondence_distance={num(self.maximum_correspondence_distance)},"
+                f"\niteration_number={self.iteration_number:d},\ntuple_scale={num(self.tuple_scale)},"
+                f"\nmaximum_tuple_count={self.maximum_tuple_count:d},\ntuple_test={b(self.tuple_test)},\n)")
+
+    def _c(self):
+        from ...._lib import FgrOption
+        for name in ("iteration_number", "maximum_tuple_count"):
+            v = getattr(self, name)
+            if not -2 ** 31 <= v < 2 ** 31:
+                raise TypeError(f"FastGlobalRegistrationOption: {name} must fit in a 32-bit int (got {v})")
+        return FgrOption(self.division_factor, int(self.use_absolute_scale), int(self.decrease_mu),
+                         self.maximum_correspondence_distance, self.iteration_number, self.tuple_scale,
+                         self.maximum_tuple_count, int(self.tuple_test))
+
+
+def _registration_fgr(source, target, corres, source_feature, target_feature, option):
+    """o3db_registration_fgr -> (RegistrationResult, FgrStats)."""
+    from ...._lib import FgrStats
+    # upstream binds both functions with "option"_a = FastGlobalRegistrationOption() built by the C++ constructor,
+    # whose decrease_mu is true, unlike the Python class's default (FastGlobalRegistration.h:48-56)
+    option = FastGlobalRegistrationOption(decrease_mu=True) if option is None else option
+    opt = option._c()
+    s = source._positions_f32("FastGlobalRegistration")
+    t = target._positions_f32("FastGlobalRegistration")
+    n, m = int(s.shape[0]), int(t.shape[0])
+    c = fs = ft = None
+    dim = 0
+    if corres is not None:
+        c = torch.as_tensor(corres)
+        if c.dtype not in (torch.int32, torch.int64) or c.dim() != 2 or c.shape[1] != 2:
+            raise RuntimeError(f"FastGlobalRegistration: corres must be an Int32 or Int64 [K, 2] tensor (got "
+                               f"{tuple(c.shape)} {c.dtype})")
+        c = c.to(device=s.device, dtype=torch.int64).contiguous()
+    else:
+        fs, ft = torch.as_tensor(source_feature), torch.as_tensor(target_feature)
+        for f, rows, name in ((fs, n, "source"), (ft, m, "target")):
+            if f.dtype != torch.float32 or f.dim() != 2 or f.shape[1] < 1:
+                raise RuntimeError(f"FastGlobalRegistration: the {name} feature must be a [N, D] Float32 tensor "
+                                   f"(got {tuple(f.shape)} {f.dtype})")
+            if int(f.shape[0]) != rows:
+                raise RuntimeError(f"FastGlobalRegistration: the {name} feature has {int(f.shape[0])} rows for "
+                                   f"{rows} points")
+        if fs.shape[1] != ft.shape[1]:
+            raise RuntimeError(f"FastGlobalRegistration: source and target features have different dimensions "
+                               f"({fs.shape[1]} and {ft.shape[1]})")
+        dim = int(fs.shape[1])
+        fs = fs.to(s.device).contiguous()
+        ft = ft.to(s.device).contiguous()
+    T = np.zeros(16, np.float64)
+    out = torch.empty((n,), dtype=torch.int64, device=s.device)
+    stats = FgrStats()
+    check(lib.o3db_registration_fgr(s.data_ptr(), n, t.data_ptr(), m, None if c is None else c.data_ptr(),
+                                    0 if c is None else int(c.shape[0]), None if fs is None else fs.data_ptr(),
+                                    None if ft is None else ft.data_ptr(), dim, C.byref(opt), dptr(T),
+                                    out.data_ptr() if n else None, C.byref(stats), current_stream_ptr()))
+    return RegistrationResult(T.reshape(4, 4), out, stats.inlier_rmse, stats.fitness), stats
+
+
+def registration_fgr_based_on_correspondence(source, target, corres, option=None):
+    """FastGlobalRegistrationBasedOnCorrespondence (pipelines/registration/FastGlobalRegistration.cpp:285-327),
+    run as upstream runs it on one thread, on the device (o3db_registration_fgr).  corres is an Int32 or Int64 [K, 2]
+    tensor or array of (source row, target row).  The tuple test draws from the library's random engine
+    (open3d_b200.utility.random.seed).  The result's transformation is 4x4 Float64 numpy; correspondence_set is Int64
+    [n] on the device, -1 for no match; converged and num_iterations are False and 0.  Without option the call uses
+    upstream's C++ defaults, as its binding does: those of FastGlobalRegistrationOption() except decrease_mu=True.
+    Float64 clouds, non-finite positions and pairs outside the clouds raise (DESIGN.md §4.26, §7)."""
+    return _registration_fgr(source, target, corres, None, None, option)[0]
+
+
+def registration_fgr_based_on_feature_matching(source, target, source_feature, target_feature, option=None):
+    """FastGlobalRegistrationBasedOnFeatureMatching (pipelines/registration/FastGlobalRegistration.cpp:329-391): the
+    mutual nearest feature rows (f32 distances, ties to the lowest row), then the tuple test and the optimisation as
+    registration_fgr_based_on_correspondence.  Features are [N, D] Float32 with one row per point of their cloud, as
+    compute_fpfh_feature returns them.  Without option, upstream's C++ defaults (decrease_mu=True) as above."""
+    return _registration_fgr(source, target, None, source_feature, target_feature, option)[0]
+
+
 def get_information_matrix(source, target, max_correspondence_distance, transformation):
     """GetInformationMatrix (Registration.cpp:446-485; pybind registration.get_information_matrix): 6x6 Float64 GTG
     of the target points matched by the transformed source, on the host like upstream."""
