@@ -439,6 +439,36 @@ int o3db_compute_transformation_symmetric(const float* source_dev, const float* 
 void o3db_pose_to_symmetric_transformation(const double pose_host[6], const double source_mean_host[3],
                                            const double target_mean_host[3], double transformation_host[16]);
 
+/* TransformationEstimationForDopplerICP (TransformationEstimation.h:356-425): the fields of the C++ constructor.  The
+ * C ABI applies its rules: |period| < 1e-3 returns O3DB_ERR_INVALID with "Time period too small.", and a
+ * lambda_doppler outside [0, 1] becomes 0.01.  Each kernel is L2 or Tukey (DISPATCH_DUAL_ROBUST_KERNEL_FUNCTION); another
+ * kernel returns "Unsupported method." once an iteration would use it.  transform_vehicle_to_sensor: row-major 4x4. */
+typedef struct {
+    double period;                          /* 0.1 */
+    double lambda_doppler;                  /* 0.01 */
+    int reject_dynamic_outliers;            /* 0 */
+    double doppler_outlier_threshold;       /* 2.0 */
+    int64_t outlier_rejection_min_iteration;       /* 2 */
+    int64_t geometric_robust_loss_min_iteration;   /* 0 */
+    int64_t doppler_robust_loss_min_iteration;     /* 2 */
+    o3db_robust_kernel geometric_kernel;    /* L2 */
+    o3db_robust_kernel doppler_kernel;      /* L2 */
+    double transform_vehicle_to_sensor[16]; /* identity */
+} o3db_doppler_params;
+
+/* kernel::ComputePoseDopplerICP (kernel/Registration.cpp:193-312, RegistrationCPU.cpp:336-493,
+ * RegistrationImpl.h:525-643) for a given Int64 correspondence set (-1 = none, n entries): source points, dopplers [n]
+ * and directions [n,3] (never transformed), target points and normals, all f32.  current_transform_host is the
+ * accumulated row-major 4x4 Float64 transformation (initial guess included) and `iteration` the index within the scale:
+ * they give the velocity v_s_in_S and the three switches.  Outputs as o3db_compute_pose_point_to_plane's
+ * (DecodeAndSolve6x6: O3DB_ERR_SINGULAR with upstream's message); [28] counts rejected dynamic points too. */
+int o3db_compute_pose_doppler_icp(const float* source_dev, const float* source_dopplers_dev,
+                                  const float* source_directions_dev, const float* target_dev,
+                                  const float* target_normals_dev, const int64_t* correspondences_dev, int64_t n,
+                                  const double current_transform_host[16], int64_t iteration,
+                                  const o3db_doppler_params* params, double* sums29_dev, double* pose_dev,
+                                  float* residual_host, int* inlier_count_host, void* stream);
+
 /* registration::GetInformationMatrix (registration/Registration.cpp:446-485, pybind get_information_matrix): the 6x6
  * Float64 information matrix GTG of a registration — a clone of the source is transformed, matched to the target by the
  * hybrid search (k = 1), and the Jacobians of the matched TARGET points are reduced
@@ -648,6 +678,14 @@ int o3db_icp_create_point_to_point(const float* source_dev, int64_t n, const flo
 int o3db_icp_create_symmetric(const float* source_dev, const float* source_normals_dev, int64_t n, const float* target_dev,
                               const float* target_normals_dev, int64_t m, const double init_source_to_target_host[16],
                               const o3db_icp_options* options, o3db_comm* comm, void* stream, o3db_icp** out);
+/* Same loop for TransformationEstimationForDopplerICP: the source needs Doppler values ([n] f32) and directions
+ * ([n,3] f32, in the sensor's vehicle frame, never transformed), the target normals.  Every iteration derives the
+ * velocity from the accumulated transformation and applies the switches of `params` on the device.  options->kernel is
+ * ignored (the params carry both kernels).  Single GPU only: a communicator is rejected (O3DB_ERR_INVALID). */
+int o3db_icp_create_doppler(const float* source_dev, const float* source_dopplers_dev, const float* source_directions_dev,
+                            int64_t n, const float* target_dev, const float* target_normals_dev, int64_t m,
+                            const double init_source_to_target_host[16], const o3db_icp_options* options,
+                            const o3db_doppler_params* params, o3db_comm* comm, void* stream, o3db_icp** out);
 /* Restore the state right after o3db_icp_create (source re-gathered, T = init). */
 int o3db_icp_reset(o3db_icp* icp, void* stream);
 /* Enqueue up to `iterations` ICP iterations (asynchronous, no host sync). */
@@ -677,6 +715,11 @@ int o3db_icp_symmetric(const float* source_dev, const float* source_normals_dev,
                        const float* target_normals_dev, int64_t m, const double init_source_to_target_host[16],
                        const o3db_icp_options* options, o3db_icp_result* result_host, int64_t* correspondences_dev,
                        double* per_iteration_host, void* stream);
+int o3db_icp_doppler(const float* source_dev, const float* source_dopplers_dev, const float* source_directions_dev, int64_t n,
+                     const float* target_dev, const float* target_normals_dev, int64_t m,
+                     const double init_source_to_target_host[16], const o3db_icp_options* options,
+                     const o3db_doppler_params* params, o3db_icp_result* result_host, int64_t* correspondences_dev,
+                     double* per_iteration_host, void* stream);
 int o3db_icp_colored(const float* source_dev, const float* source_colors_dev, int64_t n, const float* target_dev,
                      const float* target_normals_dev, const float* target_colors_dev,
                      const float* target_color_gradients_dev, int64_t m,

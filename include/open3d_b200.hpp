@@ -13,6 +13,8 @@
 
 #include <algorithm>
 #include <array>
+#include <cmath>
+#include <cstddef>
 #include <cstdint>
 #include <functional>
 #include <limits>
@@ -38,6 +40,8 @@ struct PointCloud {
     const float* normals = nullptr;    // device, may be null
     int64_t num_points = 0;
     const float* colors = nullptr;     // device, may be null
+    const float* dopplers = nullptr;   // device [N], may be null (the "dopplers" attribute DopplerICP reads)
+    const float* directions = nullptr; // device [N,3], may be null (the "directions" attribute)
     const float* color_gradients = nullptr;   // device, may be null ("color_gradients" attribute)
     bool HasPointPositions() const { return positions != nullptr && num_points > 0; }
     bool HasPointNormals() const { return normals != nullptr && num_points > 0; }
@@ -170,6 +174,92 @@ public:
     }
 
     RobustKernel kernel_;
+};
+
+/// TransformationEstimation.h:356-425: DICP's point-to-plane + Doppler objective, with the C++ constructor's arguments.
+/// |period| < 1e-3 throws "Time period too small."; a lambda_doppler outside [0, 1] becomes 0.01.
+class TransformationEstimationForDopplerICP {
+public:
+    explicit TransformationEstimationForDopplerICP(double period = 0.1, double lambda_doppler = 0.01,
+                                                   bool reject_dynamic_outliers = false,
+                                                   double doppler_outlier_threshold = 2.0,
+                                                   std::size_t outlier_rejection_min_iteration = 2,
+                                                   std::size_t geometric_robust_loss_min_iteration = 0,
+                                                   std::size_t doppler_robust_loss_min_iteration = 2,
+                                                   const RobustKernel& geometric_kernel = RobustKernel(),
+                                                   const RobustKernel& doppler_kernel = RobustKernel(),
+                                                   const std::array<double, 16>& transform_vehicle_to_sensor =
+                                                           {{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}})
+        : period_(period),
+          lambda_doppler_((lambda_doppler < 0 || lambda_doppler > 1.0) ? 0.01 : lambda_doppler),
+          reject_dynamic_outliers_(reject_dynamic_outliers),
+          doppler_outlier_threshold_(doppler_outlier_threshold),
+          outlier_rejection_min_iteration_(outlier_rejection_min_iteration),
+          geometric_robust_loss_min_iteration_(geometric_robust_loss_min_iteration),
+          doppler_robust_loss_min_iteration_(doppler_robust_loss_min_iteration),
+          geometric_kernel_(geometric_kernel),
+          doppler_kernel_(doppler_kernel),
+          transform_vehicle_to_sensor_(transform_vehicle_to_sensor) {
+        if (std::abs(period) < 1e-3) throw std::runtime_error("Time period too small.");
+    }
+
+    o3db_doppler_params Params() const {
+        o3db_doppler_params p{};
+        p.period = period_;
+        p.lambda_doppler = lambda_doppler_;
+        p.reject_dynamic_outliers = reject_dynamic_outliers_ ? 1 : 0;
+        p.doppler_outlier_threshold = doppler_outlier_threshold_;
+        p.outlier_rejection_min_iteration = static_cast<int64_t>(outlier_rejection_min_iteration_);
+        p.geometric_robust_loss_min_iteration = static_cast<int64_t>(geometric_robust_loss_min_iteration_);
+        p.doppler_robust_loss_min_iteration = static_cast<int64_t>(doppler_robust_loss_min_iteration_);
+        p.geometric_kernel = {static_cast<int>(geometric_kernel_.type_), geometric_kernel_.scaling_parameter_,
+                              geometric_kernel_.shape_parameter_};
+        p.doppler_kernel = {static_cast<int>(doppler_kernel_.type_), doppler_kernel_.scaling_parameter_,
+                            doppler_kernel_.shape_parameter_};
+        for (int i = 0; i < 16; ++i) p.transform_vehicle_to_sensor[i] = transform_vehicle_to_sensor_[i];
+        return p;
+    }
+
+    static void CheckInputs(const geometry::PointCloud& source, const geometry::PointCloud& target) {
+        if (!target.HasPointPositions() || !source.HasPointPositions())
+            throw std::runtime_error("Source and/or Target pointcloud is empty.");
+        if (!target.HasPointNormals()) throw std::runtime_error("Target pointcloud missing normals attribute.");
+        if (source.dopplers == nullptr) throw std::runtime_error("Source pointcloud missing dopplers attribute.");
+        if (source.directions == nullptr) throw std::runtime_error("Source pointcloud missing directions attribute.");
+    }
+
+    /// kernel::ComputePoseDopplerICP + PoseToTransformation (TransformationEstimation.cpp:469-519) for iteration
+    /// `iteration` of the accumulated transformation current_transform: the row-major 4x4 Float64 update.  pose_dev
+    /// and copy_to_host as TransformationEstimationPointToPlane::ComputeTransformation's.
+    std::array<double, 16> ComputeTransformation(const geometry::PointCloud& source, const geometry::PointCloud& target,
+                                                 const int64_t* correspondences_dev,
+                                                 const std::array<double, 16>& current_transform, std::size_t iteration,
+                                                 double* pose_dev,
+                                                 const std::function<void(void* dst, const void* src, size_t)>& copy_to_host,
+                                                 void* stream = nullptr) const {
+        CheckInputs(source, target);
+        const o3db_doppler_params p = Params();
+        Check(o3db_compute_pose_doppler_icp(source.positions, source.dopplers, source.directions, target.positions,
+                                            target.normals, correspondences_dev, source.num_points, current_transform.data(),
+                                            static_cast<int64_t>(iteration), &p, nullptr, pose_dev, nullptr, nullptr,
+                                            stream));
+        double pose[6];
+        copy_to_host(pose, pose_dev, sizeof(pose));
+        std::array<double, 16> T;
+        o3db_pose_to_transformation(pose, T.data());
+        return T;
+    }
+
+    double period_;
+    double lambda_doppler_;
+    bool reject_dynamic_outliers_;
+    double doppler_outlier_threshold_;
+    std::size_t outlier_rejection_min_iteration_;
+    std::size_t geometric_robust_loss_min_iteration_;
+    std::size_t doppler_robust_loss_min_iteration_;
+    RobustKernel geometric_kernel_;
+    RobustKernel doppler_kernel_;
+    std::array<double, 16> transform_vehicle_to_sensor_;
 };
 
 /// TransformationEstimation.h:318-395 (lambda_geometric outside [0,1] falls back to 0.968, :337-340)
@@ -326,6 +416,40 @@ inline RegistrationResult ICP(const geometry::PointCloud& source, const geometry
     Check(o3db_icp_symmetric(source.positions, source.normals, source.num_points, target.positions, target.normals,
                              target.num_points, init_source_to_target.data(), &opt, &r, correspondences_dev, per.data(),
                              stream));
+    return ToRegistrationResult(r, per, correspondences_dev, callback_after_iteration);
+}
+
+/// registration::ICP for TransformationEstimationForDopplerICP: the source needs dopplers and directions (never
+/// transformed), the target normals.  Single scale, as the other overloads.
+inline RegistrationResult ICP(const geometry::PointCloud& source, const geometry::PointCloud& target,
+                              double max_correspondence_distance, const std::array<double, 16>& init_source_to_target,
+                              const TransformationEstimationForDopplerICP& estimation,
+                              const ICPConvergenceCriteria& criteria = ICPConvergenceCriteria(), double voxel_size = -1.0,
+                              const IterationCallback& callback_after_iteration = nullptr,
+                              int64_t* correspondences_dev = nullptr, void* stream = nullptr) {
+    if (!target.HasPointPositions() || !source.HasPointPositions())
+        throw std::runtime_error("Source and/or Target pointcloud is empty.");
+    if (!target.HasPointNormals()) throw std::runtime_error("DopplerICP requires target pointcloud to have normals.");
+    if (source.dopplers == nullptr)
+        throw std::runtime_error("DopplerICP requires source pointcloud to have Doppler velocities.");
+    if (source.directions == nullptr)
+        throw std::runtime_error("DopplerICP requires source pointcloud to have pre-computed direction vectors.");
+    if (max_correspondence_distance <= 0.0)
+        throw std::runtime_error(" Max correspondence distance must be greater than 0, but got " +
+                                 std::to_string(max_correspondence_distance) + " in scale: 0.");
+    if (voxel_size > 0)
+        throw std::runtime_error("voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample)");
+    o3db_icp_options opt{};
+    opt.max_correspondence_distance = max_correspondence_distance;
+    opt.max_iteration = criteria.max_iteration_;
+    opt.relative_fitness = criteria.relative_fitness_;
+    opt.relative_rmse = criteria.relative_rmse_;
+    const o3db_doppler_params p = estimation.Params();
+    o3db_icp_result r{};
+    std::vector<double> per(2 * static_cast<size_t>(criteria.max_iteration_ > 0 ? criteria.max_iteration_ : 1), 0.0);
+    Check(o3db_icp_doppler(source.positions, source.dopplers, source.directions, source.num_points, target.positions,
+                           target.normals, target.num_points, init_source_to_target.data(), &opt, &p, &r,
+                           correspondences_dev, per.data(), stream));
     return ToRegistrationResult(r, per, correspondences_dev, callback_after_iteration);
 }
 

@@ -31,6 +31,15 @@ class RobustKernel(C.Structure):
     _fields_ = [("method", C.c_int), ("scale", C.c_double), ("shape", C.c_double)]
 
 
+class DopplerParams(C.Structure):
+    """o3db_doppler_params: TransformationEstimationForDopplerICP's fields."""
+    _fields_ = [("period", C.c_double), ("lambda_doppler", C.c_double), ("reject_dynamic_outliers", C.c_int),
+                ("doppler_outlier_threshold", C.c_double), ("outlier_rejection_min_iteration", C.c_int64),
+                ("geometric_robust_loss_min_iteration", C.c_int64), ("doppler_robust_loss_min_iteration", C.c_int64),
+                ("geometric_kernel", RobustKernel), ("doppler_kernel", RobustKernel),
+                ("transform_vehicle_to_sensor", C.c_double * 16)]
+
+
 class IcpOptions(C.Structure):
     _fields_ = [("max_correspondence_distance", C.c_double), ("max_iteration", C.c_int),
                 ("relative_fitness", C.c_double), ("relative_rmse", C.c_double),
@@ -160,6 +169,12 @@ _SIGS = {
                                        C.POINTER(_vp)]),
     "o3db_icp_symmetric": (_i, [_vp, _vp, _i64, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions), C.POINTER(IcpResult), _vp,
                                 _dp, _vp]),
+    "o3db_compute_pose_doppler_icp": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _dp, _i64, C.POINTER(DopplerParams),
+                                           _vp, _vp, C.POINTER(_f), C.POINTER(_i), _vp]),
+    "o3db_icp_create_doppler": (_i, [_vp, _vp, _vp, _i64, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions),
+                                     C.POINTER(DopplerParams), _vp, _vp, C.POINTER(_vp)]),
+    "o3db_icp_doppler": (_i, [_vp, _vp, _vp, _i64, _vp, _vp, _i64, _dp, C.POINTER(IcpOptions), C.POINTER(DopplerParams),
+                              C.POINTER(IcpResult), _vp, _dp, _vp]),
     "o3db_get_information_matrix": (_i, [_vp, _i64, _vp, _i64, _dbl, _dp, _dp, _vp]),
     "o3db_compute_information_matrix": (_i, [_vp, _vp, _i64, _dp, _vp, _vp]),
     "o3db_icp_reset": (_i, [_vp, _vp]),

@@ -1,5 +1,5 @@
 // icp.cu — correspondence search, pose reduction and the fused device-resident
-// ICP loop (point-to-plane, coloured, point-to-point, symmetric) for sm_90a.  See include/open3d_b200.h for the
+// ICP loop (point-to-plane, coloured, point-to-point, symmetric, Doppler) for sm_90a.  See include/open3d_b200.h for the
 // reference interfaces each entry point replaces and DESIGN.md for the design.
 //
 // No CPU fallback: every entry point needs a CUDA device.
@@ -169,9 +169,22 @@ struct SrcBlockedT {
         static_assert(PLANES == 8, "only the symmetric record carries normals");
         return reinterpret_cast<float*>(chunk(i) + 640 + 128 * axis) + (i & 31);
     }
+    // component `axis` of source direction i, and its Doppler value (9-plane records only)
+    __device__ __forceinline__ float* direction(int axis, int i) const {
+        static_assert(PLANES == 9, "only the Doppler record carries directions");
+        return reinterpret_cast<float*>(chunk(i) + 640 + 128 * axis) + (i & 31);
+    }
+    __device__ __forceinline__ float* doppler(int i) const {
+        static_assert(PLANES == 9, "only the Doppler record carries Doppler values");
+        return reinterpret_cast<float*>(chunk(i) + 1024) + (i & 31);
+    }
 };
 using SrcBlocked = SrcBlockedT<5>;
 using SrcBlockedSym = SrcBlockedT<8>;
+// The Doppler estimator's record has four more planes than the plain one, the source directions and Doppler values
+// [dx | dy | dz | doppler] (9 planes, 1152 B, 36 B per point).  They are written once, at creation, and never move:
+// PointCloud::Transform moves only positions and normals.
+using SrcBlockedDop = SrcBlockedT<9>;
 
 // no seeds, no clearances (and zeroed padding points and normals)
 template <int PLANES>
@@ -184,6 +197,10 @@ __global__ void src_blocked_init_kernel(SrcBlockedT<PLANES> sb, int64_t n, int64
         for (int axis = 0; axis < 3; ++axis) *sb.coord(axis, (int)i) = 0.f;
         if constexpr (PLANES == 8)
             for (int axis = 0; axis < 3; ++axis) *sb.normal(axis, (int)i) = 0.f;
+        if constexpr (PLANES == 9) {
+            for (int axis = 0; axis < 3; ++axis) *sb.direction(axis, (int)i) = 0.f;
+            *sb.doppler((int)i) = 0.f;
+        }
     }
 }
 
@@ -209,6 +226,17 @@ __global__ void scatter_source_kernel(const float* __restrict__ pts, const float
         *sb.normal(2, (int)p) = T.m[8] * a + T.m[9] * b + T.m[10] * c;
     }
     src_idx[p] = (int)i;
+}
+
+// the Doppler record's direction and Doppler planes, by sorted position (src_idx: sorted position -> original index);
+// both as the caller gave them: the initial transform moves neither
+__global__ void scatter_doppler_planes_kernel(const float* __restrict__ dirs, const float* __restrict__ dops, int64_t n,
+                                              const int* __restrict__ src_idx, SrcBlockedDop sb) {
+    const int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    const int64_t i = src_idx[p];
+    for (int axis = 0; axis < 3; ++axis) *sb.direction(axis, (int)p) = dirs[3 * i + axis];
+    *sb.doppler((int)p) = dops[i];
 }
 
 template <bool TRANSFORM>
@@ -682,6 +710,127 @@ __device__ __forceinline__ void accumulate_colored(float (&acc)[NACC], const Rob
 // intensity of an RGB triple exactly as upstream: float sum, divided by the double literal 3.0
 __device__ __forceinline__ float color_intensity(float r, float g, float b) { return (float)((r + g + b) / 3.0); }
 
+// ------------------------------------------------------------- Doppler ICP
+
+// TransformationEstimationForDopplerICP's constants, at the types ComputePoseDopplerICP (kernel/Registration.cpp:193-265)
+// and ComputePoseDopplerICPCPU (RegistrationCPU.cpp:427-466) give them to the per-point code.
+struct DopplerConst {
+    float R[9];          // R_S_to_V: the f64 inverse of the calibration's rotation block, cast to f32 (row-major)
+    float r[3];          // r_v_to_s_in_V: the calibration's translation column, cast to f32
+    float period;        // (float)period, the divisor of the velocities
+    float sqrt_lg;       // sqrt(1.0 - (float)lambda_doppler), rounded to f32
+    float sqrt_ld;       // sqrt(lambda_doppler), rounded to f32
+    float sqrt_ld_dt;    // sqrt_ld / (float)period in f32
+    float threshold;     // (float)doppler_outlier_threshold
+    int reject;          // reject_dynamic_outliers
+    int min_reject, min_geo, min_dop;   // the three switch iterations (clamped to INT_MAX)
+    Robust geo, dop;     // the configured kernels (L2 or Tukey: DISPATCH_DUAL_ROBUST_KERNEL_FUNCTION)
+};
+
+// What one iteration's Doppler terms read besides the record: v_s_in_S and the three switches of iteration `iter`.
+struct DopplerIter {
+    float v[3];          // v_s_in_S
+    int reject;          // dynamic-outlier rejection on
+    int method_g, method_d;   // the robust kernels in force (L2 before their switch iteration)
+};
+
+__device__ __forceinline__ float dot3_rn(float a0, float a1, float a2, float b0, float b1, float b2) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(a0, b0), __fmul_rn(a1, b1)), __fmul_rn(a2, b2));
+}
+
+// The host part of ComputePoseDopplerICP for iteration `iter` and the accumulated f64 transformation T (initial guess
+// included), in two parts.  doppler_angle: angle j of TransformationToPose (TransformationConverterImpl.h:47-60) in f64
+// without contraction, one atan2 per call so that three threads share the three.  doppler_from_angles: the pose cast to
+// f32, w = -pose[0:3] / period and v = -pose[3:6] / period in f32, then PreComputeForDopplerICP
+// (RegistrationImpl.h:525-541): v_s_in_S = R_S_to_V (v + w x r_v_to_s_in_V), f32 op by op; and the three switches.
+__device__ __forceinline__ double doppler_angle(const double* T, int j) {
+    const double sy = sqrt(__dadd_rn(__dmul_rn(T[0], T[0]), __dmul_rn(T[4], T[4])));
+    const bool big = !(sy < 1e-6);
+    double y, x;
+    if (j == 0) {
+        y = big ? T[9] : -T[6];
+        x = big ? T[10] : T[5];
+    } else if (j == 1) {
+        y = -T[8];
+        x = sy;
+    } else {
+        if (!big) return 0.0;
+        y = T[4];
+        x = T[0];
+    }
+    return atan2(y, x);
+}
+
+__device__ __forceinline__ DopplerIter doppler_from_angles(const DopplerConst& k, const double* ang, const double* T,
+                                                          int iter) {
+    const float s[6] = {(float)ang[0], (float)ang[1], (float)ang[2], (float)T[3], (float)T[7], (float)T[11]};
+    float w[3], v[3];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        w[j] = __fdiv_rn(-s[j], k.period);
+        v[j] = __fdiv_rn(-s[3 + j], k.period);
+    }
+    const float c[3] = {__fadd_rn(__fsub_rn(__fmul_rn(w[1], k.r[2]), __fmul_rn(w[2], k.r[1])), v[0]),
+                        __fadd_rn(__fsub_rn(__fmul_rn(w[2], k.r[0]), __fmul_rn(w[0], k.r[2])), v[1]),
+                        __fadd_rn(__fsub_rn(__fmul_rn(w[0], k.r[1]), __fmul_rn(w[1], k.r[0])), v[2])};
+    DopplerIter it;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) it.v[j] = dot3_rn(k.R[3 * j], k.R[3 * j + 1], k.R[3 * j + 2], c[0], c[1], c[2]);
+    it.reject = k.reject && iter >= k.min_reject;                      // kernel/Registration.cpp:222-235
+    it.method_g = iter >= k.min_geo ? k.geo.method : (int)O3DB_ROBUST_L2;
+    it.method_d = iter >= k.min_dop ? k.dop.method : (int)O3DB_ROBUST_L2;
+    return it;
+}
+
+// GetJacobianDopplerICP (RegistrationImpl.h:557-643) and the body of ComputePoseDopplerICPKernelCPU
+// (RegistrationCPU.cpp:336-400) for one correspondence: f32 op by op in the reference's order.  The Doppler error is
+// formed in f32 and widened to f64 as upstream, and r_D = (float)(sqrt_ld * error).  The direction d is the caller's,
+// never transformed.  A rejected dynamic point counts as a correspondence with zero J and r: it adds only its count.
+template <bool L2LOSS, int NACC>
+__device__ __forceinline__ void accumulate_doppler(float (&acc)[NACC], const DopplerConst& k, const DopplerIter& it,
+                                                   float sx, float sy, float sz, float tx, float ty, float tz, float nx,
+                                                   float ny, float nz, float dx, float dy, float dz, float dop) {
+    const float* R = k.R;
+    const float dsx = dot3_rn(R[0], R[1], R[2], dx, dy, dz), dsy = dot3_rn(R[3], R[4], R[5], dx, dy, dz),
+                dsz = dot3_rn(R[6], R[7], R[8], dx, dy, dz);
+    const float pred = -dot3_rn(dsx, dsy, dsz, it.v[0], it.v[1], it.v[2]);
+    const double err = (double)__fsub_rn(dop, pred);
+    if (it.reject && fabs(err) > (double)k.threshold) {
+        acc[28] += 1.0f;
+        return;
+    }
+    const float c = k.sqrt_ld_dt;
+    float JD[6];
+    JD[0] = __fmul_rn(c, __fsub_rn(__fmul_rn(dy, k.r[2]), __fmul_rn(dz, k.r[1])));
+    JD[1] = __fmul_rn(c, __fsub_rn(__fmul_rn(dz, k.r[0]), __fmul_rn(dx, k.r[2])));
+    JD[2] = __fmul_rn(c, __fsub_rn(__fmul_rn(dx, k.r[1]), __fmul_rn(dy, k.r[0])));
+    JD[3] = __fmul_rn(c, -dx);
+    JD[4] = __fmul_rn(c, -dy);
+    JD[5] = __fmul_rn(c, -dz);
+    const float rD = (float)((double)k.sqrt_ld * err);
+    const float g = k.sqrt_lg;
+    float JG[6];
+    JG[0] = __fmul_rn(g, __fadd_rn(-__fmul_rn(sz, ny), __fmul_rn(sy, nz)));
+    JG[1] = __fmul_rn(g, __fsub_rn(__fmul_rn(sz, nx), __fmul_rn(sx, nz)));
+    JG[2] = __fmul_rn(g, __fadd_rn(-__fmul_rn(sy, nx), __fmul_rn(sx, ny)));
+    JG[3] = __fmul_rn(g, nx);
+    JG[4] = __fmul_rn(g, ny);
+    JG[5] = __fmul_rn(g, nz);
+    const float rG = __fmul_rn(g, dot3_rn(__fsub_rn(sx, tx), __fsub_rn(sy, ty), __fsub_rn(sz, tz), nx, ny, nz));
+    const float wG = L2LOSS ? 1.0f : robust_weight(Robust{it.method_g, k.geo.scale, k.geo.shape}, rG);
+    const float wD = L2LOSS ? 1.0f : robust_weight(Robust{it.method_d, k.dop.scale, k.dop.shape}, rD);
+    int q = 0;
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+        const float gw = __fmul_rn(JG[j], wG), dw = __fmul_rn(JD[j], wD);
+#pragma unroll
+        for (int l = 0; l <= j; ++l) acc[q++] += __fadd_rn(__fmul_rn(gw, JG[l]), __fmul_rn(dw, JD[l]));
+        acc[21 + j] += __fadd_rn(__fmul_rn(gw, rG), __fmul_rn(dw, rD));
+    }
+    acc[27] += __fadd_rn(__fmul_rn(rG, rG), __fmul_rn(rD, rD));
+    acc[28] += 1.0f;
+}
+
 // -------------------------------------------- stand-alone pose reductions
 
 struct PoseOut {
@@ -866,6 +1015,37 @@ symmetric_means_kernel(const float* __restrict__ src, const float* __restrict__ 
     if (threadIdx.x < kNumSums) out[threadIdx.x] = s_final[threadIdx.x];
 }
 
+struct Mat4d {
+    double m[16];
+};
+
+// ComputePoseDopplerICPKernelCPU (RegistrationCPU.cpp:336-400) for iteration `iter` of the transformation T: thread 0 of
+// each block derives the velocity and the switches (doppler_iteration, the fused loop's own derivation), then the
+// 29 sums and the pose as pose_p2plane_kernel.
+template <bool L2LOSS>
+__global__ void __launch_bounds__(kThreads)
+pose_doppler_kernel(const float* __restrict__ src, const float* __restrict__ dops, const float* __restrict__ dirs,
+                    const float* __restrict__ tgt, const float* __restrict__ nrm, const int64_t* __restrict__ corr, int64_t n,
+                    const __grid_constant__ DopplerConst k, const __grid_constant__ Mat4d T, int iter, double* __restrict__ partials, unsigned* ticket, PoseOut out) {
+    __shared__ double s_warp[kThreads / 32][kSumStride];
+    __shared__ double s_final[kSumStride];
+    __shared__ double s_ang[3];
+    if (threadIdx.x < 3) s_ang[threadIdx.x] = doppler_angle(T.m, threadIdx.x);
+    __syncthreads();
+    const DopplerIter it = doppler_from_angles(k, s_ang, T.m, iter);
+    if (!reduce_sums(n, s_warp, partials, ticket, s_final, [&](int64_t i, float (&acc)[kNumSums]) {
+            const int64_t c = corr[i];
+            if (c == -1) return;
+            const float* t = tgt + 3 * c;
+            const float* m = nrm + 3 * c;
+            const float* d = dirs + 3 * i;
+            accumulate_doppler<L2LOSS, kNumSums>(acc, k, it, src[3 * i], src[3 * i + 1], src[3 * i + 2], t[0], t[1], t[2],
+                                                 m[0], m[1], m[2], d[0], d[1], d[2], dops[i]);
+        }))
+        return;
+    pose_epilogue(s_final, out);
+}
+
 // ComputeInformationMatrixKernelCUDA (RegistrationCUDA.cu:492-533) with GetInformationJacobians (RegistrationImpl.h:686-715):
 // the 21 lower-triangle terms of GTG per matched target point (f32, upstream's expression), reduced like the pose sums
 // (f32 per thread over a few terms, then f64: deterministic, and closer to the exact sum than upstream's f32 atomics).
@@ -937,10 +1117,10 @@ __global__ void pack_source_intensity_kernel(const int* __restrict__ src_idx, co
 // ------------------------------------------------------------ fused ICP loop
 
 // The estimator of a handle: which per-query terms an iteration adds and which step turns the totals into an update.
-enum : int { kEstPlane = 0, kEstColored = 1, kEstPoint = 2, kEstSymmetric = 3 };
+enum : int { kEstPlane = 0, kEstColored = 1, kEstPoint = 2, kEstSymmetric = 3, kEstDoppler = 4 };
 // the working source's record of an estimator's kernels (SrcBlockedT)
 template <int EST>
-using SrcOf = SrcBlockedT<EST == kEstSymmetric ? 8 : 5>;
+using SrcOf = SrcBlockedT<EST == kEstSymmetric ? 8 : EST == kEstDoppler ? 9 : 5>;
 
 struct IcpState {        // lives in device memory; read back once at the end
     double T[16];        // cumulative source->target transformation (f64)
@@ -955,6 +1135,10 @@ struct IcpState {        // lives in device memory; read back once at the end
     int status;          // 0 ok, 1 singular
     unsigned ticket;
     int sums_cached;     // chunk_sums holds every chunk's line for the working source as it is now (see IcpArgs)
+    // Doppler only: the velocity and switches of the next iteration (doppler_iteration, written by the finalize warp),
+    // and whether they equal the previous iteration's bit for bit (the condition of sum replay besides the points)
+    DopplerIter dop;
+    int dop_same;
 };
 
 struct IcpArgs {
@@ -993,6 +1177,8 @@ struct IcpArgs {
     // symmetric only: the second sum line (sum of s, sum of t; reduce.cuh) per 32-query chunk (8 floats) and per block
     float* chunk_sums2;
     double* partials2;
+    // Doppler only: the estimator's constants (the kernels in force come from st->dop)
+    DopplerConst dop;
 };
 
 __device__ void set_identity(double* T, float* Uf) {
@@ -1008,6 +1194,24 @@ __device__ void set_identity(double* T, float* Uf) {
 // and a third of the block prologues / epilogues; the loop itself has no block-wide barrier either way.  On an H100
 // it is 3-6 % faster than three 256-thread blocks per SM (profiles/h100_reduce_ab.jsonl).
 static constexpr int kIcpThreads = 768;
+
+// ComputePoseDopplerICP's inputs for the iteration st->iter with st->T, and whether they repeat the last iteration's.
+// By one warp (all 32 lanes), after the step has written T and iter; `scratch`: 3 doubles of shared memory.
+__device__ __forceinline__ void doppler_advance_warp(const DopplerConst& k, IcpState* st, double* scratch) {
+    const int lane = threadIdx.x & 31;
+    __syncwarp();
+    if (lane < 3) scratch[lane] = doppler_angle(st->T, lane);
+    __syncwarp();
+    if (lane == 0) {
+        const DopplerIter it = doppler_from_angles(k, scratch, st->T, st->iter);
+        const DopplerIter& old = st->dop;
+        st->dop_same = __float_as_uint(it.v[0]) == __float_as_uint(old.v[0]) &&
+                       __float_as_uint(it.v[1]) == __float_as_uint(old.v[1]) &&
+                       __float_as_uint(it.v[2]) == __float_as_uint(old.v[2]) && it.reject == old.reject &&
+                       it.method_g == old.method_g && it.method_d == old.method_d;
+        st->dop = it;
+    }
+}
 
 // Host part of DoSingleScaleICPIterations (Registration.cpp:293-358), on device, run by ONE WARP once per
 // iteration (all 32 lanes must call it): gauss_newton_step_warp and left_multiply_warp (reduce.cuh) spread the
@@ -1103,6 +1307,13 @@ struct SymQuery {
     float nrm[3];
     float acc2[kSymLine2];
 };
+// The Doppler estimator's query also reads its direction and Doppler value (from the record) and the iteration's
+// velocity and switches (shared memory).
+struct DopQuery {
+    float dir[3];
+    float dop;
+    const DopplerIter* it;
+};
 
 // transform_normals_kernel's expression: the rotation block of the pending update
 __device__ __forceinline__ void rotate_normal(const float* __restrict__ T, float& x, float& y, float& z) {
@@ -1115,7 +1326,8 @@ __device__ __forceinline__ void rotate_normal(const float* __restrict__ T, float
 template <bool L2LOSS, int MODE, int EST>
 __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float* s_U, int i, float px, float py, float pz,
                                                   int jp, float clear_prev, const float4* seed_ts, const float4* seed_nn,
-                                                  const float4* seed_cg, float (&acc)[32], SymQuery* sym = nullptr) {
+                                                  const float4* seed_cg, float (&acc)[32], SymQuery* sym = nullptr,
+                                                  const DopQuery* dq = nullptr) {
     const SrcOf<EST> src{a.src.base};
     const float ox = px, oy = py, oz = pz;
     apply_transform(s_U, px, py, pz);
@@ -1197,6 +1409,9 @@ __device__ __forceinline__ bool icp_process_query(const IcpArgs& a, const float*
                 const float ns[3] = {sym->nrm[0], sym->nrm[1], sym->nrm[2]}, nt[3] = {nn.x, nn.y, nn.z};
                 accumulate_symmetric<L2LOSS>(acc, sym->acc2, vs, vt, ns, nt,
                                              [&](float r) { return robust_weight(a.rk, r); });
+            } else if constexpr (EST == kEstDoppler) {
+                accumulate_doppler<L2LOSS, 32>(acc, a.dop, *dq->it, px, py, pz, t.x, t.y, t.z, nn.x, nn.y, nn.z, dq->dir[0],
+                                               dq->dir[1], dq->dir[2], dq->dop);
             } else {
                 accumulate_p2plane<L2LOSS, 32>(acc, a.rk, px, py, pz, t.x, t.y, t.z, nn.x, nn.y, nn.z);
             }
@@ -1349,8 +1564,11 @@ __device__ __forceinline__ void icp_block_epilogue(const IcpArgs& a, double (*s_
                 }
                 return;
             }
-            if (MODE == 0) icp_finalize_iteration<EST>(a, s_final, sums2, &s_warp[0][0]);   // (s_warp is dead: reused as scratch)
-            else if (threadIdx.x == 0) icp_finalize_evaluate(a, s_final);
+            if (MODE == 0) {
+                icp_finalize_iteration<EST>(a, s_final, sums2, &s_warp[0][0]);   // (s_warp is dead: reused as scratch)
+                if constexpr (EST == kEstDoppler)   // the next iteration's velocity, from T as the step left it
+                    doppler_advance_warp(a.dop, a.st, &s_warp[0][0]);
+            } else if (threadIdx.x == 0) icp_finalize_evaluate(a, s_final);
         }
     } else if (threadIdx.x < kNumSums) {
         a.st->sums[threadIdx.x] = s_final[threadIdx.x];
@@ -1395,6 +1613,20 @@ struct __align__(16) IcpStage<kEstSymmetric> {
     float4 ns[32];
     float4 cg[1];
 };
+// The Doppler stage: its A part is the 9-plane record (SrcBlockedDop), 1152 bytes, still ONE bulk copy.
+template <>
+struct __align__(16) IcpStage<kEstDoppler> {
+    float px[32];
+    float py[32];
+    float pz[32];
+    int jp[32];
+    float d2[32];
+    float dir[3][32];   // source directions
+    float dop[32];      // Doppler values
+    float4 ts[32];
+    float4 ns[32];
+    float4 cg[1];
+};
 
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* b) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
@@ -1415,6 +1647,11 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 template <int EST>
 struct IcpStagedSmem {   // dynamic shared memory of the iteration kernels
     IcpStage<EST> stage[kIcpThreads / 32][2];
+};
+template <>
+struct IcpStagedSmem<kEstDoppler> {   // and the iteration's velocity and switches
+    IcpStage<kEstDoppler> stage[kIcpThreads / 32][2];
+    DopplerIter it;
 };
 
 // The body of every iteration kernel below: one source for the ring, the search, the replay and the epilogue.
@@ -1438,7 +1675,13 @@ __device__ __forceinline__ void icp_iteration(const IcpArgs& a) {
     if (threadIdx.x == 0) {
         s_done = *(volatile int*)&a.st->done;
         s_reverse = a.st->executed & 1;
-        s_cached = MODE == 0 && a.st->sums_cached;
+        if constexpr (EST == kEstDoppler) {
+            // the Doppler terms also read the velocity and the switches: a chunk replays only while they repeat too
+            s_cached = MODE == 0 && a.st->sums_cached && a.st->dop_same;
+            sm.it = a.st->dop;
+        } else {
+            s_cached = MODE == 0 && a.st->sums_cached;
+        }
     }
     if (threadIdx.x < 16) s_U[threadIdx.x] = a.st->Uf[threadIdx.x];
     __syncthreads();
@@ -1464,6 +1707,9 @@ __device__ __forceinline__ void icp_iteration(const IcpArgs& a) {
                   offsetof(IcpStage<EST>, jp) == 384 && offsetof(IcpStage<EST>, d2) == 512 &&
                   offsetof(IcpStage<EST>, ts) == kBytesA, "stage A mirrors a chunk record");
     if constexpr (kSym) static_assert(offsetof(IcpStage<EST>, sn) == 640, "stage A mirrors the symmetric record");
+    if constexpr (EST == kEstDoppler)
+        static_assert(offsetof(IcpStage<EST>, dir) == 640 && offsetof(IcpStage<EST>, dop) == 1024,
+                      "stage A mirrors the Doppler record");
     // chunk c (the warp's c-th step) covers working-source positions [start + c * step, ... + 32)
     auto issue_a = [&](int c) {                // lane 0: ONE TMA bulk copy of chunk c's record into slot c & 1
         if (lane == 0 && c < steps) {
@@ -1543,6 +1789,13 @@ __device__ __forceinline__ void icp_iteration(const IcpArgs& a) {
 #pragma unroll
             for (int k = 0; k < 3; ++k) sym.nrm[k] = sl.sn[k][lane];
         }
+        DopQuery dq;
+        if constexpr (EST == kEstDoppler) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) dq.dir[k] = sl.dir[k][lane];
+            dq.dop = sl.dop[lane];
+            dq.it = &sm.it;
+        }
         __syncwarp();          // every lane has read its point / jp / d2 of slot c & 1: hand that part back to the producer
         issue_a(c + 2);
         issue_b(c + 1);
@@ -1565,7 +1818,7 @@ __device__ __forceinline__ void icp_iteration(const IcpArgs& a) {
         if (i < n)
             matched = icp_process_query<L2LOSS, MODE, EST>(a, s_U, i, px, py, pz, jp, clear_prev, &sl.ts[lane],
                                                            &sl.ns[EST == kEstPoint ? 0 : lane],
-                                                           &sl.cg[EST == kEstColored ? lane : 0], term, &sym);
+                                                           &sl.cg[EST == kEstColored ? lane : 0], term, &sym, &dq);
         const float line = icp_accumulate_chunk(term, matched, acc64);
         if (MODE == 0) a.chunk_sums[q0 + lane] = line;   // one coalesced 128-byte store
         if constexpr (kSym && MODE == 0) {   // the second line: same rules (+0.0 when no lane matched)
@@ -1602,7 +1855,21 @@ icp_symmetric_iteration_kernel(const __grid_constant__ IcpArgs a) {
     icp_iteration<L2LOSS, MODE, kEstSymmetric>(a);
 }
 
-// Multi-GPU: runs after the all-reduce of st->sums.  (Symmetric handles take no communicator.)
+// The Doppler iteration and its evaluation pass (the 9-plane record: not icp_iteration_kernel<true, 1> either).
+template <bool L2LOSS, int MODE>
+__global__ void __launch_bounds__(kIcpThreads, 1)
+icp_doppler_iteration_kernel(const __grid_constant__ IcpArgs a) {
+    icp_iteration<L2LOSS, MODE, kEstDoppler>(a);
+}
+
+// The velocity and switches of a Doppler handle's first iteration, from its initial transformation.  <<<1, 32>>>
+__global__ void doppler_init_kernel(const __grid_constant__ IcpArgs a) {
+    __shared__ double s_ang[3];
+    doppler_advance_warp(a.dop, a.st, s_ang);
+    if (threadIdx.x == 0) a.st->dop_same = 0;
+}
+
+// Multi-GPU: runs after the all-reduce of st->sums.  (Symmetric and Doppler handles take no communicator.)
 template <int MODE>
 __global__ void icp_finalize_kernel(IcpArgs a) {   // <<<1, 32>>>
     __shared__ double s_scratch[64];
@@ -1658,6 +1925,11 @@ struct o3db_icp {
     const float* src_normals_user = nullptr;
     o3db::DevPtr<float> chunk_sums2;    // n_pad / 4 floats: 8 per 32-query chunk
     o3db::DevPtr<double> partials2;     // grid_blocks x 8
+    // TransformationEstimationForDopplerICP: 9-plane records carrying the source directions and Doppler values
+    bool doppler = false;
+    const float* src_dopplers_user = nullptr;
+    const float* src_directions_user = nullptr;
+    o3db::DopplerConst dop{};
 };
 
 namespace o3db {
@@ -1665,6 +1937,9 @@ namespace o3db {
 typedef void (*IcpKernel)(IcpArgs);
 // mode 0 = iterate (loss / colour of the handle), 1 = final evaluation (no Jacobian)
 static IcpKernel icp_kernel_for(const o3db_icp* c, int mode) {
+    if (c->doppler)
+        return mode == 1 ? icp_doppler_iteration_kernel<true, 1>
+                         : c->l2loss ? icp_doppler_iteration_kernel<true, 0> : icp_doppler_iteration_kernel<false, 0>;
     if (c->symmetric)
         return mode == 1 ? icp_symmetric_iteration_kernel<true, 1>
                          : c->l2loss ? icp_symmetric_iteration_kernel<true, 0> : icp_symmetric_iteration_kernel<false, 0>;
@@ -1677,6 +1952,7 @@ static IcpKernel icp_kernel_for(const o3db_icp* c, int mode) {
 // dynamic shared memory of the handle's iteration kernels (the stage ring)
 static size_t icp_smem_bytes(const o3db_icp* c, int mode) {
     if (c->symmetric) return sizeof(IcpStagedSmem<kEstSymmetric>);
+    if (c->doppler) return sizeof(IcpStagedSmem<kEstDoppler>);
     if (mode == 1) return sizeof(IcpStagedSmem<kEstPlane>);
     return c->colored ? sizeof(IcpStagedSmem<kEstColored>) : c->point ? sizeof(IcpStagedSmem<kEstPoint>) : sizeof(IcpStagedSmem<kEstPlane>);
 }
@@ -1725,6 +2001,7 @@ static IcpArgs make_args(o3db_icp* c) {
     for (int k = 0; k < 3; ++k) a.pivot[k] = c->pivot[k];
     a.chunk_sums2 = c->chunk_sums2.get();
     a.partials2 = c->partials2.get();
+    a.dop = c->dop;
     return a;
 }
 
@@ -1739,10 +2016,16 @@ static int icp_init_state(o3db_icp* c, cudaStream_t st) {
     const unsigned nb = (unsigned)ceil_div(c->n_pad, kThreads);
     if (c->symmetric)
         src_blocked_init_kernel<<<nb, kThreads, 0, st>>>(SrcBlockedSym{c->src_blk.get()}, c->n, c->n_pad, false);
+    else if (c->doppler)
+        src_blocked_init_kernel<<<nb, kThreads, 0, st>>>(SrcBlockedDop{c->src_blk.get()}, c->n, c->n_pad, false);
     else
         src_blocked_init_kernel<<<nb, kThreads, 0, st>>>(SrcBlocked{c->src_blk.get()}, c->n, c->n_pad,
                                                          false);   // no seeds, no clearances
     O3DB_LAUNCH_CHECK();
+    if (c->doppler) {   // the first iteration's velocity, on the device like every later one
+        doppler_init_kernel<<<1, 32, 0, st>>>(make_args(c));
+        O3DB_LAUNCH_CHECK();
+    }
     c->launched = 0;
     return O3DB_OK;
 }
@@ -1756,10 +2039,18 @@ static int icp_gather_source(o3db_icp* c, cudaStream_t st) {
         scatter_source_kernel<<<nb, kThreads, 0, st>>>(c->src_user, c->src_normals_user, c->n, T0, c->src_start.get(),
                                                        c->src_key.get(), c->src_rank.get(), SrcBlockedSym{c->src_blk.get()},
                                                        c->src_idx.get());
+    else if (c->doppler)
+        scatter_source_kernel<<<nb, kThreads, 0, st>>>(c->src_user, nullptr, c->n, T0, c->src_start.get(), c->src_key.get(),
+                                                       c->src_rank.get(), SrcBlockedDop{c->src_blk.get()}, c->src_idx.get());
     else
         scatter_source_kernel<<<nb, kThreads, 0, st>>>(c->src_user, nullptr, c->n, T0, c->src_start.get(), c->src_key.get(),
                                                        c->src_rank.get(), SrcBlocked{c->src_blk.get()}, c->src_idx.get());
     O3DB_LAUNCH_CHECK();
+    if (c->doppler) {
+        scatter_doppler_planes_kernel<<<nb, kThreads, 0, st>>>(c->src_directions_user, c->src_dopplers_user, c->n,
+                                                               c->src_idx.get(), SrcBlockedDop{c->src_blk.get()});
+        O3DB_LAUNCH_CHECK();
+    }
     return O3DB_OK;
 }
 
@@ -2121,6 +2412,100 @@ int o3db_compute_transformation_symmetric(const float* source_dev, const float* 
     return O3DB_OK;
 }
 
+}  // extern "C"
+
+namespace o3db {
+
+// TransformationEstimationForDopplerICP's constructor rules (TransformationEstimation.h:406-425) and the host part of
+// ComputePoseDopplerICP (kernel/Registration.cpp:212-235, RegistrationCPU.cpp:450-456) -> the kernels' constants.
+static int doppler_const(const o3db_doppler_params* p, int max_iteration, DopplerConst* k) {
+    O3DB_REQUIRE(p != nullptr, "DopplerICP: null parameters");
+    if (!(std::fabs(p->period) >= 1e-3)) {   // kMinTimePeriod
+        set_last_error("Time period too small.");
+        return O3DB_ERR_INVALID;
+    }
+    const double lambda = (p->lambda_doppler < 0 || p->lambda_doppler > 1.0) ? 0.01 : p->lambda_doppler;
+    // DISPATCH_DUAL_ROBUST_KERNEL_FUNCTION (RobustKernelImpl.h:122-185) dispatches L2 and Tukey only, and raises once
+    // an iteration uses another kernel
+    const o3db_robust_kernel* ks[2] = {&p->geometric_kernel, &p->doppler_kernel};
+    const int64_t mins[2] = {p->geometric_robust_loss_min_iteration, p->doppler_robust_loss_min_iteration};
+    for (int j = 0; j < 2; ++j)
+        if (ks[j]->method != O3DB_ROBUST_L2 && ks[j]->method != O3DB_ROBUST_TUKEY && mins[j] < max_iteration) {
+            set_last_error("Unsupported method.");
+            return O3DB_ERR_INVALID;
+        }
+    // R_S_to_V: the f64 inverse of the 3x3 block (Gauss-Jordan, partial pivoting), cast to f32
+    const double* C = p->transform_vehicle_to_sensor;
+    double M[3][6];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 6; ++j) M[i][j] = j < 3 ? C[4 * i + j] : (j - 3 == i ? 1.0 : 0.0);
+    for (int col = 0; col < 3; ++col) {
+        int piv = col;
+        for (int i = col + 1; i < 3; ++i)
+            if (std::fabs(M[i][col]) > std::fabs(M[piv][col])) piv = i;
+        if (!(M[piv][col] != 0.0) || !std::isfinite(M[piv][col])) {
+            set_last_error("DopplerICP: the rotation block of transform_vehicle_to_sensor is singular.");
+            return O3DB_ERR_INVALID;
+        }
+        for (int j = 0; j < 6; ++j) std::swap(M[col][j], M[piv][j]);
+        const double d = M[col][col];
+        for (int j = 0; j < 6; ++j) M[col][j] /= d;
+        for (int i = 0; i < 3; ++i)
+            if (i != col) {
+                const double f = M[i][col];
+                for (int j = 0; j < 6; ++j) M[i][j] -= f * M[col][j];
+            }
+    }
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) k->R[3 * i + j] = (float)M[i][3 + j];
+        k->r[i] = (float)C[4 * i + 3];
+    }
+    k->period = (float)p->period;
+    k->sqrt_lg = (float)std::sqrt(1.0 - (double)(float)lambda);
+    k->sqrt_ld = (float)std::sqrt(lambda);
+    k->sqrt_ld_dt = k->sqrt_ld / k->period;
+    k->threshold = (float)p->doppler_outlier_threshold;
+    k->reject = p->reject_dynamic_outliers ? 1 : 0;
+    const auto clamp = [](int64_t v) { return (int)std::min<int64_t>(std::max<int64_t>(v, 0), INT_MAX); };
+    k->min_reject = clamp(p->outlier_rejection_min_iteration);
+    k->min_geo = clamp(p->geometric_robust_loss_min_iteration);
+    k->min_dop = clamp(p->doppler_robust_loss_min_iteration);
+    k->geo = Robust{ks[0]->method, (float)ks[0]->scale, ks[0]->shape};
+    k->dop = Robust{ks[1]->method, (float)ks[1]->scale, ks[1]->shape};
+    return O3DB_OK;
+}
+
+}  // namespace o3db
+
+extern "C" {
+
+int o3db_compute_pose_doppler_icp(const float* source_dev, const float* source_dopplers_dev,
+                                  const float* source_directions_dev, const float* target_dev,
+                                  const float* target_normals_dev, const int64_t* correspondences_dev, int64_t n,
+                                  const double current_transform_host[16], int64_t iteration,
+                                  const o3db_doppler_params* params, double* sums29_dev, double* pose_dev,
+                                  float* residual_host, int* inlier_count_host, void* stream) {
+    O3DB_REQUIRE(n >= 0 && current_transform_host && iteration >= 0 &&
+                         (n == 0 || (source_dev && source_dopplers_dev && source_directions_dev && target_dev &&
+                                     target_normals_dev && correspondences_dev)),
+                 "o3db_compute_pose_doppler_icp: bad arguments");
+    // only the iteration's kernels must be dispatchable: validate as for a loop that ends after it
+    DopplerConst k;
+    if (int rc = doppler_const(params, (int)std::min<int64_t>(iteration + 1, INT_MAX), &k)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    PoseScratch s;
+    if (int rc = pose_scratch_alloc(&s, n, st)) return rc;
+    Mat4d T;
+    memcpy(T.m, current_transform_host, sizeof(T.m));
+    const int iter = (int)std::min<int64_t>(iteration, INT_MAX);
+    const bool l2 = (iter < k.min_geo || k.geo.method == O3DB_ROBUST_L2) && (iter < k.min_dop || k.dop.method == O3DB_ROBUST_L2);
+    (l2 ? pose_doppler_kernel<true> : pose_doppler_kernel<false>)<<<s.blocks, kThreads, 0, st>>>(
+            source_dev, source_dopplers_dev, source_directions_dev, target_dev, target_normals_dev, correspondences_dev, n, k,
+            T, iter, s.partials, s.ticket, PoseOut{s.sums, pose_dev, s.status});
+    O3DB_LAUNCH_CHECK();
+    return pose_finish(&s, sums29_dev, residual_host, inlier_count_host, st);
+}
+
 int o3db_compute_information_matrix(const float* target_dev, const int64_t* correspondences_dev, int64_t n,
                                     double information_host[36], int64_t* num_correspondences_host, void* stream) {
     O3DB_REQUIRE(target_dev && correspondences_dev && information_host && n > 0, "o3db_compute_information_matrix: bad arguments");
@@ -2183,6 +2568,9 @@ struct EstimatorInputs {   // all device pointers; null source_colors and source
                            // point-to-plane
     bool point_to_point = false;   // no target normals wanted
     const float* source_normals = nullptr;   // symmetric
+    const float* source_dopplers = nullptr;   // Doppler (with source_directions and dop)
+    const float* source_directions = nullptr;
+    const DopplerConst* dop = nullptr;
     const float* source_colors = nullptr;
     const float* target_colors = nullptr;
     const float* target_color_gradients = nullptr;
@@ -2214,7 +2602,12 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     c->point = col.point_to_point;
     c->symmetric = col.source_normals != nullptr;
     c->src_normals_user = col.source_normals;
-    c->l2loss = c->point || options->kernel.method == O3DB_ROBUST_L2;
+    c->doppler = col.dop != nullptr;
+    c->src_dopplers_user = col.source_dopplers;
+    c->src_directions_user = col.source_directions;
+    if (col.dop) c->dop = *col.dop;
+    c->l2loss = c->point || (col.dop ? col.dop->geo.method == O3DB_ROBUST_L2 && col.dop->dop.method == O3DB_ROBUST_L2
+                                     : options->kernel.method == O3DB_ROBUST_L2);
     c->colored = col.source_colors != nullptr;
     c->src_colors_user = col.source_colors;
     c->lambda_geometric = col.lambda_geometric;
@@ -2239,7 +2632,8 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     c->src_keys = ncell;
     // padded to whole 256-entry chunks: the staged kernel copies 32-entry chunks with TMA bulk copies
     c->n_pad = ceil_div(n, 256) * 256;
-    if ((rc = dev_alloc(c->src_blk, c->symmetric ? SrcBlockedSym::bytes(c->n_pad) : SrcBlocked::bytes(c->n_pad), st)))
+    if ((rc = dev_alloc(c->src_blk, c->symmetric ? SrcBlockedSym::bytes(c->n_pad)
+                                    : c->doppler ? SrcBlockedDop::bytes(c->n_pad) : SrcBlocked::bytes(c->n_pad), st)))
         return rc;
     if ((rc = dev_alloc(c->src_idx, (size_t)c->n_pad, st))) return rc;
     // (no initial contents: IcpState::sums_cached starts at 0, so the first iteration writes every line)
@@ -2248,6 +2642,9 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
         if ((rc = dev_alloc(c->chunk_sums2, (size_t)(c->n_pad / 32) * kSymLine2, st))) return rc;
         if ((rc = dev_alloc(c->partials2, (size_t)c->grid_blocks * kSymLine2, st))) return rc;
         src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlockedSym{c->src_blk.get()},
+                                                                                           n, c->n_pad, true);
+    } else if (c->doppler) {
+        src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlockedDop{c->src_blk.get()},
                                                                                            n, c->n_pad, true);
     } else {
         src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlocked{c->src_blk.get()}, n,
@@ -2362,6 +2759,30 @@ int o3db_icp_create_symmetric(const float* source_dev, const float* source_norma
     return icp_create_impl(source_dev, n, target_dev, target_normals_dev, m, init_T, options, nullptr, est, stream, out);
 }
 
+int o3db_icp_create_doppler(const float* source_dev, const float* source_dopplers_dev, const float* source_directions_dev,
+                            int64_t n, const float* target_dev, const float* target_normals_dev, int64_t m,
+                            const double init_T[16], const o3db_icp_options* options, const o3db_doppler_params* params,
+                            o3db_comm* comm, void* stream, o3db_icp** out) {
+    O3DB_REQUIRE(out != nullptr, "o3db_icp_create_doppler: out is null");
+    *out = nullptr;
+    O3DB_REQUIRE(options != nullptr, "o3db_icp_create: null options / init");
+    // Registration.cpp:180-197 and TransformationEstimation.cpp:469-481
+    O3DB_REQUIRE(source_dev && target_dev && n > 0 && m > 0, "Source and/or Target pointcloud is empty.");
+    O3DB_REQUIRE(target_normals_dev != nullptr, "DopplerICP requires target pointcloud to have normals.");
+    O3DB_REQUIRE(source_dopplers_dev != nullptr, "DopplerICP requires source pointcloud to have Doppler velocities.");
+    O3DB_REQUIRE(source_directions_dev != nullptr,
+                 "DopplerICP requires source pointcloud to have pre-computed direction vectors.");
+    // the in-kernel exchange and the NCCL path would need every rank's velocity derivation to agree; not built
+    O3DB_REQUIRE(comm == nullptr, "DopplerICP does not run multi-GPU: pass no communicator.");
+    o3db::DopplerConst k;
+    if (int rc = o3db::doppler_const(params, options->max_iteration, &k)) return rc;
+    o3db::EstimatorInputs est;
+    est.source_dopplers = source_dopplers_dev;
+    est.source_directions = source_directions_dev;
+    est.dop = &k;
+    return icp_create_impl(source_dev, n, target_dev, target_normals_dev, m, init_T, options, nullptr, est, stream, out);
+}
+
 int o3db_icp_reset(o3db_icp* c, void* stream) {
     O3DB_REQUIRE(c != nullptr, "o3db_icp_reset: null handle");
     cudaStream_t st = (cudaStream_t)stream;
@@ -2470,6 +2891,21 @@ int o3db_icp_symmetric(const float* source_dev, const float* source_normals_dev,
     o3db_icp* c = nullptr;
     int rc = o3db_icp_create_symmetric(source_dev, source_normals_dev, n, target_dev, target_normals_dev, m, init_T, options,
                                        nullptr, stream, &c);
+    if (rc) return rc;
+    rc = o3db_icp_iterate(c, options->max_iteration, stream);
+    if (rc == O3DB_OK) rc = o3db_icp_finish(c, result, correspondences_dev, per_iteration_host, stream);
+    cudaStreamSynchronize((cudaStream_t)stream);
+    o3db_icp_destroy(c);
+    return rc;
+}
+
+int o3db_icp_doppler(const float* source_dev, const float* source_dopplers_dev, const float* source_directions_dev, int64_t n,
+                     const float* target_dev, const float* target_normals_dev, int64_t m, const double init_T[16],
+                     const o3db_icp_options* options, const o3db_doppler_params* params, o3db_icp_result* result,
+                     int64_t* correspondences_dev, double* per_iteration_host, void* stream) {
+    o3db_icp* c = nullptr;
+    int rc = o3db_icp_create_doppler(source_dev, source_dopplers_dev, source_directions_dev, n, target_dev,
+                                     target_normals_dev, m, init_T, options, params, nullptr, stream, &c);
     if (rc) return rc;
     rc = o3db_icp_iterate(c, options->max_iteration, stream);
     if (rc == O3DB_OK) rc = o3db_icp_finish(c, result, correspondences_dev, per_iteration_host, stream);

@@ -1,5 +1,5 @@
-"""Mirror of ``open3d.t.pipelines.registration`` for the point-to-point, point-to-plane, symmetric and coloured ICP paths
-(cpp/pybind/t/pipelines/registration/registration.cpp:96-140, 469-530;
+"""Mirror of ``open3d.t.pipelines.registration`` for the point-to-point, point-to-plane, symmetric, coloured and Doppler
+ICP paths (cpp/pybind/t/pipelines/registration/registration.cpp:96-140, 469-530;
 cpp/open3d/t/pipelines/registration/{Registration,TransformationEstimation}.cpp).
 
 The iteration loop itself runs device-resident inside libo3db200.so
@@ -18,7 +18,8 @@ import numpy as np
 import torch
 
 from ... import geometry as _geometry
-from ...._lib import (ERR_SINGULAR, IcpOptions, IcpResult, O3DBError, RobustKernel as _CRobust, check, dptr, lib)
+from ...._lib import (ERR_SINGULAR, DopplerParams, IcpOptions, IcpResult, O3DBError, RobustKernel as _CRobust, check, dptr,
+                      lib)
 from ....core import as_device_f32_points, as_host_f64_4x4, current_stream_ptr
 
 PointCloud = _geometry.PointCloud
@@ -324,6 +325,127 @@ class TransformationEstimationSymmetric(TransformationEstimation):
         return T
 
 
+class TransformationEstimationForDopplerICP(TransformationEstimation):
+    """TransformationEstimation.h:356-470 / TransformationEstimation.cpp:434-523: point-to-plane ICP plus the FMCW
+    Doppler term of DICP (Hexsel, Vhavle and Chen, RSS 2022), energy (1 - lambda) E_G + lambda E_D.  The source needs
+    "dopplers" ([N] or [N, 1] Float32, radial velocities) and "directions" ([N, 3] Float32, unit rays in the vehicle
+    frame, never transformed), the target normals.  The arguments are the C++ constructor's; upstream's one-argument
+    Python overload, which passes its value to `period`, is not reproduced.  Each kernel is L2 or Tukey, the two that
+    upstream's dual dispatch accepts."""
+
+    def __init__(self, period: float = 0.1, lambda_doppler: float = 0.01, reject_dynamic_outliers: bool = False,
+                 doppler_outlier_threshold: float = 2.0, outlier_rejection_min_iteration: int = 2,
+                 geometric_robust_loss_min_iteration: int = 0, doppler_robust_loss_min_iteration: int = 2,
+                 geometric_kernel: RobustKernel | None = None, doppler_kernel: RobustKernel | None = None,
+                 transform_vehicle_to_sensor=None):
+        T = np.eye(4) if transform_vehicle_to_sensor is None else transform_vehicle_to_sensor
+        if isinstance(T, torch.Tensor):
+            T = T.detach().cpu().numpy()
+        T = np.asarray(T, np.float64)
+        if T.shape != (4, 4):   # core::AssertTensorShape(transform_vehicle_to_sensor, {4, 4})
+            raise RuntimeError(f"Tensor has shape {list(T.shape)}, but is expected to have [4, 4].")
+        if abs(period) < 1e-3:   # kMinTimePeriod
+            raise RuntimeError("Time period too small.")
+        if lambda_doppler < 0 or lambda_doppler > 1.0:
+            lambda_doppler = 0.01
+        self.period = float(period)
+        self.lambda_doppler = float(lambda_doppler)
+        self.reject_dynamic_outliers = bool(reject_dynamic_outliers)
+        self.doppler_outlier_threshold = float(doppler_outlier_threshold)
+        self.outlier_rejection_min_iteration = int(outlier_rejection_min_iteration)
+        self.geometric_robust_loss_min_iteration = int(geometric_robust_loss_min_iteration)
+        self.doppler_robust_loss_min_iteration = int(doppler_robust_loss_min_iteration)
+        self.geometric_kernel = geometric_kernel if geometric_kernel is not None else RobustKernel()
+        self.doppler_kernel = doppler_kernel if doppler_kernel is not None else RobustKernel()
+        self.transform_vehicle_to_sensor = T.copy()
+
+    @property
+    def kernel(self):   # the search options' kernel slot (the Doppler handle reads both kernels from _params)
+        return self.geometric_kernel
+
+    def __repr__(self):
+        return f"TransformationEstimationForDopplerICP with lambda_doppler: {self.lambda_doppler:f}"
+
+    def _params(self):
+        p = DopplerParams()
+        p.period, p.lambda_doppler = float(self.period), float(self.lambda_doppler)
+        p.reject_dynamic_outliers = int(bool(self.reject_dynamic_outliers))
+        p.doppler_outlier_threshold = float(self.doppler_outlier_threshold)
+        p.outlier_rejection_min_iteration = int(self.outlier_rejection_min_iteration)
+        p.geometric_robust_loss_min_iteration = int(self.geometric_robust_loss_min_iteration)
+        p.doppler_robust_loss_min_iteration = int(self.doppler_robust_loss_min_iteration)
+        p.geometric_kernel, p.doppler_kernel = self.geometric_kernel._c(), self.doppler_kernel._c()
+        T = np.asarray(self.transform_vehicle_to_sensor, np.float64)
+        if T.shape != (4, 4):
+            raise RuntimeError(f"Tensor has shape {list(T.shape)}, but is expected to have [4, 4].")
+        p.transform_vehicle_to_sensor[:] = [float(v) for v in T.reshape(16)]
+        return p
+
+    @staticmethod
+    def _check(source, target):
+        """TransformationEstimation.cpp:469-499 (and the positions' dtype, which every estimator here requires)."""
+        if not source.has_point_positions() or not target.has_point_positions():
+            raise RuntimeError("Source and/or Target pointcloud is empty.")
+        if not target.has_point_normals():
+            raise RuntimeError("Target pointcloud missing normals attribute.")
+        if "dopplers" not in source.point:
+            raise RuntimeError("Source pointcloud missing dopplers attribute.")
+        if "directions" not in source.point:
+            raise RuntimeError("Source pointcloud missing directions attribute.")
+        return TransformationEstimationForDopplerICP._doppler_inputs(source)
+
+    @staticmethod
+    def _doppler_inputs(source):
+        """(dopplers [N], directions [N, 3]) as contiguous Float32 on the device; raises on any other dtype or shape."""
+        s, d, r = source.point["positions"], source.point["dopplers"], source.point["directions"]
+        n = s.shape[0]
+        for name, v in (("positions", s), ("dopplers", d), ("directions", r)):
+            if v.dtype != torch.float32:
+                raise RuntimeError(f"DopplerICP: source {name} must be Float32, got {v.dtype} (Float64 clouds are not "
+                                   "supported).")
+        if not (tuple(d.shape) == (n,) or tuple(d.shape) == (n, 1)):
+            raise RuntimeError(f"DopplerICP: source dopplers must have shape [{n}] or [{n}, 1], got {list(d.shape)}.")
+        if tuple(r.shape) != (n, 3):
+            raise RuntimeError(f"DopplerICP: source directions must have shape [{n}, 3], got {list(r.shape)}.")
+        return d.reshape(-1).cuda().contiguous(), r.cuda().contiguous()
+
+    def compute_rmse(self, source, target, correspondences):
+        """TransformationEstimation.cpp:434-467: the point-to-plane RMSE over the valid pairs (torch ops on the
+        device, tensor ops upstream)."""
+        self._check(source, target)
+        s, t, n = source.point["positions"], target.point["positions"], target.point["normals"]
+        corr = _corr_arg(correspondences, s.shape[0])
+        valid = corr != -1
+        idx = corr[valid]
+        e = ((s[valid] - t[idx]) * n[idx]) ** 2
+        return float(torch.sqrt(e.sum(dtype=torch.float64) / idx.shape[0]))
+
+    def compute_pose(self, source, target, correspondences, current_transform=None, iteration=0):
+        """kernel::ComputePoseDopplerICP (kernel/Registration.cpp:193-312) through the C ABI seam
+        o3db_compute_pose_doppler_icp: pose [6] f64 on the device, residual, inlier_count and the 29 sums."""
+        dops, dirs = self._check(source, target)
+        s, t, n = source.point["positions"], target.point["positions"], target.point["normals"]
+        corr = _corr_arg(correspondences, s.shape[0])
+        T = as_host_f64_4x4(np.eye(4) if current_transform is None else current_transform, "current_transform")
+        pose = torch.zeros(6, dtype=torch.float64, device=s.device)
+        sums = torch.zeros(29, dtype=torch.float64, device=s.device)
+        residual, count = C.c_float(0), C.c_int(0)
+        p = self._params()
+        check(lib.o3db_compute_pose_doppler_icp(s.data_ptr(), dops.data_ptr(), dirs.data_ptr(), t.data_ptr(),
+                                                n.data_ptr(), corr.data_ptr(), s.shape[0], dptr(T), int(iteration),
+                                                C.byref(p), sums.data_ptr(), pose.data_ptr(), C.byref(residual),
+                                                C.byref(count), current_stream_ptr()))
+        return pose, float(residual.value), int(count.value), sums
+
+    def compute_transformation(self, source, target, correspondences, current_transform=None, iteration=0):
+        """TransformationEstimation.cpp:469-519 -> 4x4 Float64 on CPU (PoseToTransformation of the seam's pose)."""
+        pose, _, _, _ = self.compute_pose(source, target, correspondences, current_transform, iteration)
+        p = np.ascontiguousarray(pose.cpu().numpy())
+        T = np.zeros((4, 4), np.float64)
+        lib.o3db_pose_to_transformation(dptr(p), dptr(T))
+        return T
+
+
 def pose_to_symmetric_transformation(pose, source_mean, target_mean):
     """kernel::PoseToSymmetricTransformation (TransformationConverter.cpp:106-133, SymmetricICPImpl.h:19-43) on the
     host in f64 -> 4x4."""
@@ -351,9 +473,11 @@ def _assert_inputs(source, target, estimation_method, max_correspondence_distanc
     colored = isinstance(estimation_method, TransformationEstimationForColoredICP)
     if not colored and not isinstance(estimation_method, (TransformationEstimationPointToPoint,
                                                           TransformationEstimationPointToPlane,
-                                                          TransformationEstimationSymmetric)):
-        raise RuntimeError("open3d_b200 implements TransformationEstimationPointToPoint, ...Symmetric, ...PointToPlane "
-                           "and ...ForColoredICP; other estimators are outside this build's scope (SURVEY.md §8f).")
+                                                          TransformationEstimationSymmetric,
+                                                          TransformationEstimationForDopplerICP)):
+        raise RuntimeError("open3d_b200 implements TransformationEstimationPointToPoint, ...Symmetric, ...ForDopplerICP, "
+                           "...PointToPlane and ...ForColoredICP; other estimators are outside this build's scope "
+                           "(SURVEY.md §8f).")
     if not target.has_point_positions() or not source.has_point_positions():
         raise RuntimeError("Source and/or Target pointcloud is empty.")
     if colored:
@@ -368,6 +492,14 @@ def _assert_inputs(source, target, estimation_method, max_correspondence_distanc
                            "PointCloud.")
     elif isinstance(estimation_method, TransformationEstimationSymmetric):
         TransformationEstimationSymmetric._check(source, target)
+    elif isinstance(estimation_method, TransformationEstimationForDopplerICP):
+        if not target.has_point_normals():
+            raise RuntimeError("DopplerICP requires target pointcloud to have normals.")
+        if "dopplers" not in source.point:
+            raise RuntimeError("DopplerICP requires source pointcloud to have Doppler velocities.")
+        if "directions" not in source.point:
+            raise RuntimeError("DopplerICP requires source pointcloud to have pre-computed direction vectors.")
+        TransformationEstimationForDopplerICP._doppler_inputs(source)
     if max_correspondence_distance <= 0.0:
         raise RuntimeError(" Max correspondence distance must be greater than 0, but got "
                            f"{max_correspondence_distance} in scale: {scale_idx}.")
@@ -410,6 +542,12 @@ def _run_single_scale(source, target, max_dist, init, estimation, criteria, call
             ns, nt = source.point["normals"], target.point["normals"]
             check(lib.o3db_icp_create_symmetric(s.data_ptr(), ns.data_ptr(), s.shape[0], t.data_ptr(), nt.data_ptr(),
                                                 t.shape[0], dptr(T0), C.byref(opt), None, stream, C.byref(handle)))
+        elif isinstance(estimation, TransformationEstimationForDopplerICP):
+            dops, dirs = estimation._check(source, target)
+            nt, p = target.point["normals"], estimation._params()
+            check(lib.o3db_icp_create_doppler(s.data_ptr(), dops.data_ptr(), dirs.data_ptr(), s.shape[0], t.data_ptr(),
+                                              nt.data_ptr(), t.shape[0], dptr(T0), C.byref(opt), C.byref(p), None,
+                                              stream, C.byref(handle)))
         else:
             n = target.point["normals"]
             check(lib.o3db_icp_create(s.data_ptr(), s.shape[0], t.data_ptr(), n.data_ptr(), t.shape[0], dptr(T0),
@@ -835,6 +973,20 @@ def _replicate_from_rank0(cloud, comm):
     return out
 
 
+def _doppler_voxel_down_sample(cloud, voxel_size):
+    """A Doppler source's pyramid level: positions, directions and Doppler values averaged per voxel, as upstream's
+    VoxelDownSample averages every attribute (PointCloud.cpp:536-552).  voxel_down_sample averages [N, 3] attributes,
+    so the Doppler values ride as the first column of one; the directions are averaged, not renormalised, as upstream."""
+    dops, dirs = TransformationEstimationForDopplerICP._doppler_inputs(cloud)
+    tmp = PointCloud()
+    tmp.point["positions"] = cloud.point["positions"]
+    tmp.point["directions"] = dirs
+    tmp.point["dopplers3"] = torch.nn.functional.pad(dops[:, None], (0, 2))
+    out = tmp.voxel_down_sample(voxel_size)
+    out.point["dopplers"] = out.point.pop("dopplers3")[:, 0].contiguous()
+    return out
+
+
 def multi_scale_icp(source, target, voxel_sizes, criteria_list, max_correspondence_distances,
                     init_source_to_target=None, estimation_method=None, callback_after_iteration=None, comm=None):
     """MultiScaleICP (Registration.cpp:362-444).
@@ -848,6 +1000,8 @@ def multi_scale_icp(source, target, voxel_sizes, criteria_list, max_corresponden
     if comm is not None and isinstance(estimation_method, TransformationEstimationSymmetric):
         # the multi-GPU exchange carries the 30 sums of one line; this estimator also sums both clouds' points
         raise RuntimeError("TransformationEstimationSymmetric does not run multi-GPU: pass comm=None.")
+    if comm is not None and isinstance(estimation_method, TransformationEstimationForDopplerICP):
+        raise RuntimeError("TransformationEstimationForDopplerICP does not run multi-GPU: pass comm=None.")
     n_scales = len(criteria_list)
     if len(voxel_sizes) != n_scales or len(max_correspondence_distances) != n_scales:
         raise RuntimeError(" [MultiScaleICP]: Size of criterias, voxel_size, max_correspondence_distances vectors "
@@ -861,10 +1015,12 @@ def multi_scale_icp(source, target, voxel_sizes, criteria_list, max_corresponden
             raise RuntimeError(" [MultiScaleICP]: Voxel sizes must be in strictly decreasing order.")
     # InitializePointCloudPyramidForMultiScaleICP (Registration.cpp:221-273)
     src_pyr, tgt_pyr = [None] * n_scales, [None] * n_scales
+    doppler = isinstance(estimation_method, TransformationEstimationForDopplerICP)
+    down_src = _doppler_voxel_down_sample if doppler else (lambda c, v: c.voxel_down_sample(v))
     if voxel_sizes[-1] <= 0:
         src_pyr[-1], tgt_pyr[-1] = source, target          # (the loop clones the source itself)
     else:
-        src_pyr[-1], tgt_pyr[-1] = source.voxel_down_sample(voxel_sizes[-1]), target.voxel_down_sample(voxel_sizes[-1])
+        src_pyr[-1], tgt_pyr[-1] = down_src(source, voxel_sizes[-1]), target.voxel_down_sample(voxel_sizes[-1])
     if isinstance(estimation_method, TransformationEstimationForColoredICP) and \
             "color_gradients" not in target.point:          # Registration.cpp:243-263
         if voxel_sizes[-1] <= 0:
@@ -873,7 +1029,7 @@ def multi_scale_icp(source, target, voxel_sizes, criteria_list, max_corresponden
         else:
             tgt_pyr[-1].estimate_color_gradients(30, voxel_sizes[-1] * 4.0)
     for k in range(n_scales - 2, -1, -1):
-        src_pyr[k] = src_pyr[k + 1].voxel_down_sample(voxel_sizes[k])
+        src_pyr[k] = down_src(src_pyr[k + 1], voxel_sizes[k])
         tgt_pyr[k] = tgt_pyr[k + 1].voxel_down_sample(voxel_sizes[k])
     if comm is not None and comm.world > 1:
         src_pyr = [_replicate_from_rank0(c, comm) for c in src_pyr]
