@@ -945,6 +945,29 @@ int o3db_vbg_extract_point_cloud(o3db_vbg* vbg, float weight_threshold, int64_t 
                                  float** points, float** normals, float** colors, void* stream);
 
 /* ------------------------------------------------------------------------
+ * VoxelBlockGrid::ExtractTriangleMesh (t/geometry/VoxelBlockGrid.cpp:436-472; slam::Model::ExtractTriangleMesh
+ * forwards to it) = BufferRadiusNeighbors + kernel::voxel_grid::ExtractTriangleMesh (kernel/VoxelBlockGridImpl.h:
+ * 1385-1780), marching cubes over the cubes of 8 voxels: a cube contributes when all 8 corners exist with weight >
+ * weight_threshold; its case is the 8-bit tsdf < 0 pattern (-0.0 is not negative).  The edge (o, o + e_i) gets a
+ * vertex when its corners differ in that bit and one of the up to four cubes sharing it contributes; the vertex has
+ * the point cloud's position, normal and colour expressions (a corner at exactly 0 gives a vertex at ratio 0).
+ *
+ * Vertices come in o3db_vbg_extract_point_cloud's order (block slot, voxel, axis); triangles by block slot, voxel and
+ * the case table's order, as Int32 vertex indices wound as upstream winds them.  Each case's polygons are upstream's;
+ * they may be split along other diagonals (DESIGN.md §4.27).  Two calls on an unchanged volume give identical bits.
+ * estimated_vertex_number > 0 only sizes the buffers ahead of the count: the mesh is always complete.  The surface may
+ * hold at most INT32_MAX vertices and INT32_MAX triangles.
+ *
+ * Outputs: *num_vertices, *num_triangles, [*num_vertices, 3] f32 and [*num_triangles, 3] i32 device buffers owned by
+ * the handle, valid until the next o3db_vbg_extract_triangle_mesh on it or o3db_vbg_destroy (an extract_point_cloud
+ * call does not touch them); *colors is NULL for a grid without colour, all four are NULL for an empty surface.
+ * Synchronises the stream once (the two counts); reports a frame dropped for capacity like o3db_vbg_size.
+ * ---------------------------------------------------------------------- */
+int o3db_vbg_extract_triangle_mesh(o3db_vbg* vbg, float weight_threshold, int64_t estimated_vertex_number,
+                                   int64_t* num_vertices, int64_t* num_triangles, float** vertices, float** normals,
+                                   float** colors, int32_t** triangles, void* stream);
+
+/* ------------------------------------------------------------------------
  * Point clouds from depth / RGB-D images and back (t/geometry/kernel/ paths).
  *
  * o3db_unproject: PointCloud::CreateFromDepthImage / CreateFromRGBDImage without normals (t/geometry/PointCloud.cpp:

@@ -230,6 +230,8 @@ _SIGS = {
                                _vp, _vp]),
     "o3db_vbg_extract_point_cloud": (_i, [_vp, _f, _i64, C.POINTER(_i64), C.POINTER(_vp), C.POINTER(_vp),
                                           C.POINTER(_vp), _vp]),
+    "o3db_vbg_extract_triangle_mesh": (_i, [_vp, _f, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_vp),
+                                            C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), _vp]),
     "o3db_unproject": (_i, [_vp, _i, _i, _i, _vp, _i, _dp, _dp, _f, _f, _i, _vp, _vp, C.POINTER(_i64), _vp]),
     "o3db_project": (_i, [_vp, _vp, _i64, _dp, _dp, _f, _f, _i, _i, _vp, _vp, _vp]),
     "o3db_vbg_profile": (_i, [_vp, _i]),

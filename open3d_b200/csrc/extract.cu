@@ -1,4 +1,5 @@
-// extract.cu — VoxelBlockGrid::ExtractPointCloud for sm_90a: the TSDF surface as points with normals (and colours).
+// extract.cu — VoxelBlockGrid::ExtractPointCloud for sm_90a: the TSDF surface as points with normals (and colours);
+// below it, VoxelBlockGrid::ExtractTriangleMesh, which reuses its neighbour table, vertex emission and scan.
 //
 // Reference: VoxelBlockGrid.cpp:404-434 (driver), BufferRadiusNeighbors (:22-51) and
 // kernel::voxel_grid::ExtractPointCloud (VoxelBlockGridImpl.h:1122-1381, DeviceGetLinearIdx / DeviceGetNormal :94-149).
@@ -25,6 +26,7 @@
 
 #include "common.cuh"
 #include "hash.cuh"
+#include "marching_cubes.cuh"
 #include "scan.cuh"
 #include "vbg.cuh"
 
@@ -280,6 +282,211 @@ __global__ void __launch_bounds__(kET) extract_emit_kernel(ExtractArgs a) {
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// VoxelBlockGrid::ExtractTriangleMesh (VoxelBlockGrid.cpp:436-472, kernel VoxelBlockGridImpl.h:1385-1780).  The cube
+// at voxel o has corners o + {0,1}^3; it contributes when all 8 exist with weight > threshold, and its case is the
+// 8-bit tsdf < 0 pattern (marching_cubes.cuh).  The edge (o, o + e_i) carries a vertex when one of the up to four
+// cubes sharing it contributes and its corners differ in that bit (upstream's pass 0 marking).  Vertex rows are the
+// point cloud's (extract_emit_kernel over the vertex bits, in its order); triangle rows come by block, then voxel,
+// then the generated table's order, each written reversed as upstream writes it.  Nine passes in twelve launches:
+//   neighbours   extract_neighbors_kernel;
+//   classify     one CTA per block stages the tsdf < 0 / contributing bits of voxels [0, R]^3 in shared memory and
+//                writes one case byte per cube;
+//   count        one CTA per block stages the case bytes of cubes [-1, R-1]^3, derives each owned edge's vertex bit
+//                into ballot words as extract_count_kernel does, keeps the block's vertices before each word, and
+//                writes the block's vertex and triangle counts;
+//   scan x 2     the per-block vertex and triangle counts;
+//   vertices     extract_emit_kernel;
+//   triangles    one CTA per block scans its cubes' triangle counts in voxel order; a corner's vertex is the owning
+//                block's first row + the rank of its (voxel, axis) bit in that block's words.
+
+static constexpr mc::Table kMcTable = mc::make_table();
+__constant__ mc::Table c_mc = kMcTable;
+
+struct MeshArgs {
+    ExtractArgs e;              // as the point cloud's, with the mesh's nb / counts (vertices) / masks / total
+    unsigned char* cases;
+    unsigned* wbase;
+    unsigned* tcounts;
+    unsigned long long* ttotal;
+    long long tlimit;           // triangle rows to write
+    int* triangles;
+};
+
+// Loads s[((z*(R+1)) + y)*(R+1) + x] = f(linear index of voxel (x, y, z) + lo, or -1) for x, y, z in [0, R].
+template <typename F>
+__device__ __forceinline__ void stage_halo(const ExtractArgs& a, const int* s_nb, int lo, unsigned char* s, F f) {
+    const int R = a.res, R1 = R + 1;
+    for (int h = threadIdx.x; h < R1 * R1 * R1; h += kET) {
+        const int x = h % R1, y = (h / R1) % R1, z = h / (R1 * R1);
+        s[h] = f(linear_idx(s_nb, R, a.div_res, x + lo, y + lo, z + lo));
+    }
+}
+
+__global__ void __launch_bounds__(kET) mesh_classify_kernel(MeshArgs m) {
+    extern __shared__ unsigned char s_flag[];   // [(R+1)^3] voxels [0, R]^3: bit 0 exists with weight > threshold, bit 1 tsdf < 0
+    __shared__ int s_nb[27];
+    pdl_wait();
+    const ExtractArgs& a = m.e;
+    const int n = *a.size, R = a.res, R1 = R + 1;
+    for (int b = blockIdx.x; b < n; b += gridDim.x) {
+        __syncthreads();   // the previous block's readers of s_nb and s_flag are done
+        if (threadIdx.x < 27) s_nb[threadIdx.x] = a.nb[27 * (size_t)b + threadIdx.x];
+        __syncthreads();
+        stage_halo(a, s_nb, 0, s_flag, [&](long long lin) -> unsigned char {
+            // VoxelBlockGridImpl.h:1479-1484: a missing corner or weight <= threshold leaves the cube out
+            if (lin < 0 || (float)a.weight[lin] <= a.weight_threshold) return 0;
+            return a.tsdf[lin] < 0.f ? 3 : 1;
+        });
+        __syncthreads();
+        for (int v = threadIdx.x; v < a.res3; v += kET) {
+            const int q = fast_div(v, a.div_res), z = fast_div(v, a.div_res2);
+            const int x = v - q * R, y = q - z * R;
+            unsigned all = 1, c = 0;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const unsigned f = s_flag[((z + mc::corner_offset(k, 2)) * R1 + y + mc::corner_offset(k, 1)) * R1 +
+                                                x + mc::corner_offset(k, 0)];
+                all &= f;
+                c |= (f >> 1) << k;
+            }
+            m.cases[(size_t)b * a.res3 + v] = (unsigned char)(all ? c : 0u);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kET) mesh_count_kernel(MeshArgs m) {
+    extern __shared__ unsigned char s_case[];   // [(R+1)^3] cubes at voxels [-1, R-1]^3
+    __shared__ int s_nb[27];
+    __shared__ unsigned s_warp[kET / 32];
+    pdl_wait();
+    const ExtractArgs& a = m.e;
+    const int n = *a.size, R = a.res, R1 = R + 1, R3 = a.res3;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int b = blockIdx.x; b < a.capacity; b += gridDim.x) {
+        if (b >= n) {   // the scans run over every slot
+            if (threadIdx.x == 0) a.counts[b] = m.tcounts[b] = 0;
+            continue;
+        }
+        __syncthreads();
+        if (threadIdx.x < 27) s_nb[threadIdx.x] = a.nb[27 * (size_t)b + threadIdx.x];
+        __syncthreads();
+        stage_halo(a, s_nb, -1, s_case,
+                   [&](long long lin) -> unsigned char { return lin < 0 ? 0 : m.cases[lin]; });
+        __syncthreads();
+        unsigned rows = 0, tris = 0;
+        for (int v0 = 0; v0 < a.words * 32; v0 += kET) {
+            const int v = v0 + threadIdx.x;
+            unsigned bits = 0;
+            if (v < R3) {
+                const int q = fast_div(v, a.div_res), z = fast_div(v, a.div_res2);
+                const int x = v - q * R, y = q - z * R;
+                const int h = ((z + 1) * R1 + y + 1) * R1 + x + 1;   // the cube at o
+                tris += c_mc.ntri[s_case[h]];
+                const int st[3] = {1, R1, R1 * R1};
+#pragma unroll
+                for (int i = 0; i < 3; ++i) {   // edge (o, o + e_i) as seen from the cubes at o - s
+                    unsigned cross = 0;
+#pragma unroll
+                    for (int s = 0; s < 4; ++s) {
+                        int off[3] = {0, 0, 0};
+                        off[(i + 1) % 3] = s & 1;
+                        off[(i + 2) % 3] = s >> 1;
+                        const unsigned c = s_case[h - off[0] * st[0] - off[1] * st[1] - off[2] * st[2]];
+                        const int lo = mc::corner_at(off[0], off[1], off[2]);
+                        const int hi = mc::corner_at(off[0] + (i == 0), off[1] + (i == 1), off[2] + (i == 2));
+                        cross |= (c >> lo) ^ (c >> hi);
+                    }
+                    bits |= (cross & 1u) << i;
+                }
+            }
+            const unsigned m0 = __ballot_sync(0xffffffffu, bits & 1u);
+            const unsigned m1 = __ballot_sync(0xffffffffu, bits & 2u);
+            const unsigned m2 = __ballot_sync(0xffffffffu, bits & 4u);
+            const int w = (v0 >> 5) + warp;
+            if (lane == 0) s_warp[warp] = __popc(m0) + __popc(m1) + __popc(m2);
+            __syncthreads();
+            if (lane == 0 && w < a.words) {
+                unsigned* mk = a.masks + ((size_t)b * a.words + w) * 3;
+                mk[0] = m0;
+                mk[1] = m1;
+                mk[2] = m2;
+                unsigned before = rows;
+                for (int k = 0; k < warp; ++k) before += s_warp[k];
+                m.wbase[(size_t)b * a.words + w] = before;
+            }
+#pragma unroll
+            for (int k = 0; k < kET / 32; ++k) rows += s_warp[k];
+            __syncthreads();   // s_warp is rewritten by the next round
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) tris += __shfl_xor_sync(0xffffffffu, tris, o);
+        if (lane == 0) s_warp[warp] = tris;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            unsigned t = 0;
+#pragma unroll
+            for (int k = 0; k < kET / 32; ++k) t += s_warp[k];
+            a.counts[b] = rows;
+            m.tcounts[b] = t;
+            if (rows) atomicAdd(a.total, (unsigned long long)rows);
+            if (t) atomicAdd(m.ttotal, (unsigned long long)t);
+        }
+    }
+}
+
+// The triangles of the cube at voxel v of the current block (case c, nt triangles, first row `row`), :1704-1750.
+__device__ void emit_cube(const MeshArgs& m, const int* s_nb, int v, unsigned c, unsigned nt, long long row) {
+    const ExtractArgs& a = m.e;
+    const int R = a.res;
+    const int q = fast_div(v, a.div_res), z = fast_div(v, a.div_res2);
+    const int x = v - q * R, y = q - z * R;
+    for (unsigned t = 0; t < nt; ++t, ++row) {
+        if (row >= m.tlimit) return;
+        int* tri = m.triangles + 3 * row;
+        for (int k = 0; k < 3; ++k) {
+            const unsigned ow = c_mc.owner[c_mc.tri[c][3 * t + k]];
+            const int o[3] = {x + (int)(ow & 1u), y + (int)((ow >> 1) & 1u), z + (int)((ow >> 2) & 1u)};
+            const int axis = (int)(ow >> 3);
+            const int bx = o[0] >= R, by = o[1] >= R, bz = o[2] >= R;   // owner in the +x / +y / +z neighbour
+            const int slot = s_nb[13 + bx + 3 * by + 9 * bz];
+            const int lv = ((o[2] - bz * R) * R + o[1] - by * R) * R + o[0] - bx * R, l = lv & 31;
+            const size_t wi = (size_t)slot * a.words + (lv >> 5);
+            const unsigned* mk = a.masks + 3 * wi;
+            const unsigned below = (1u << l) - 1u;
+            unsigned idx = a.counts[slot] + m.wbase[wi] + __popc(mk[0] & below) + __popc(mk[1] & below) +
+                           __popc(mk[2] & below);
+            if (axis > 0) idx += (mk[0] >> l) & 1u;
+            if (axis > 1) idx += (mk[1] >> l) & 1u;
+            tri[2 - k] = (int)idx;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kET) mesh_triangle_kernel(MeshArgs m) {
+    __shared__ int s_nb[27];
+    __shared__ unsigned s_part[kET / 32];
+    pdl_wait();
+    const ExtractArgs& a = m.e;
+    const int n = *a.size;
+    for (int b = blockIdx.x; b < n; b += gridDim.x) {
+        long long row = m.tcounts[b];
+        if (row >= m.tlimit) continue;
+        __syncthreads();   // the previous block's readers of s_nb are done
+        if (threadIdx.x < 27) s_nb[threadIdx.x] = a.nb[27 * (size_t)b + threadIdx.x];
+        __syncthreads();
+        for (int v0 = 0; v0 < a.res3; v0 += kET) {
+            const int v = v0 + threadIdx.x;
+            const unsigned c = v < a.res3 ? m.cases[(size_t)b * a.res3 + v] : 0u;
+            const unsigned nt = c_mc.ntri[c];
+            unsigned total;
+            const unsigned ex = cta_exclusive_scan(nt, s_part, total);
+            if (nt) emit_cube(m, s_nb, v, c, nt, row + ex);
+            row += total;
+        }
+    }
+}
+
 static int ensure_scratch(o3db_vbg* v, cudaStream_t st) {
     if (v->ext_blocks >= v->map.capacity) return O3DB_OK;
     for (GridPtr<unsigned>* p : {&v->ext_counts, &v->ext_scan, &v->ext_masks}) free_on(*p, st);
@@ -320,6 +527,69 @@ static int launch_emit(const o3db_vbg* v, ExtractArgs a, long long limit, unsign
     a.normals = v->ext_normals.get();
     a.colors = v->with_color ? v->ext_colors.get() : nullptr;
     O3DB_CUDA_CHECK(launch_pdl_ex(extract_emit_kernel, {grid, kET}, st, a));
+    return O3DB_OK;
+}
+
+static int ensure_mesh_scratch(o3db_vbg* v, cudaStream_t st) {
+    if (v->mesh_blocks >= v->map.capacity) return O3DB_OK;
+    for (GridPtr<unsigned>* p : {&v->mesh_vcounts, &v->mesh_tcounts, &v->mesh_scan, &v->mesh_masks, &v->mesh_wbase})
+        free_on(*p, st);
+    free_on(v->mesh_nb, st);
+    free_on(v->mesh_cases, st);
+    v->mesh_blocks = 0;
+    const int64_t cap = v->map.capacity, r3 = (int64_t)v->resolution * v->resolution * v->resolution;
+    const int64_t words = ceil_div(r3, 32);
+    if (int rc = dev_alloc(v->mesh_nb, (size_t)cap * 27, st)) return rc;
+    if (int rc = dev_alloc(v->mesh_cases, (size_t)(cap * r3), st)) return rc;
+    if (int rc = dev_alloc(v->mesh_vcounts, (size_t)(cap + 1), st)) return rc;
+    if (int rc = dev_alloc(v->mesh_tcounts, (size_t)(cap + 1), st)) return rc;
+    if (int rc = dev_alloc(v->mesh_scan, (size_t)ceil_div(cap, kScanTile), st)) return rc;
+    if (int rc = dev_alloc(v->mesh_masks, (size_t)cap * words * 3, st)) return rc;
+    if (int rc = dev_alloc(v->mesh_wbase, (size_t)cap * words, st)) return rc;
+    if (!v->mesh_totals)
+        if (int rc = dev_alloc(v->mesh_totals, 2, st)) return rc;
+    if (!v->h_mesh_totals) {
+        v->h_mesh_totals = pinned_block<long long[]>(2);
+        O3DB_REQUIRE(v->h_mesh_totals != nullptr, "o3db_vbg_extract_triangle_mesh: out of pinned host memory");
+    }
+    v->mesh_blocks = cap;
+    return O3DB_OK;
+}
+
+// Grows the vertex and triangle buffers to at least `verts` and `tris` rows, with the point cloud's headroom.
+static int ensure_mesh_rows(o3db_vbg* v, int64_t verts, int64_t tris, cudaStream_t st) {
+    const auto grow = [](int64_t r) { return std::max<int64_t>(r, std::min<int64_t>(INT_MAX, r + r / 4)); };
+    if (verts > v->mesh_vrows) {
+        for (GridPtr<float>* p : {&v->mesh_positions, &v->mesh_normals, &v->mesh_colors}) free_on(*p, st);
+        v->mesh_vrows = 0;
+        verts = grow(verts);
+        if (int rc = dev_alloc(v->mesh_positions, (size_t)verts * 3, st)) return rc;
+        if (int rc = dev_alloc(v->mesh_normals, (size_t)verts * 3, st)) return rc;
+        if (v->with_color)
+            if (int rc = dev_alloc(v->mesh_colors, (size_t)verts * 3, st)) return rc;
+        v->mesh_vrows = verts;
+    }
+    if (tris > v->mesh_trows) {
+        free_on(v->mesh_triangles, st);
+        v->mesh_trows = 0;
+        tris = grow(tris);
+        if (int rc = dev_alloc(v->mesh_triangles, (size_t)tris * 3, st)) return rc;
+        v->mesh_trows = tris;
+    }
+    return O3DB_OK;
+}
+
+// The vertex and triangle emission into the handle's mesh buffers, limited to their first `verts` and `tris` rows.
+static int launch_mesh_emit(const o3db_vbg* v, MeshArgs m, long long verts, long long tris, unsigned grid,
+                            cudaStream_t st) {
+    m.e.limit = verts;
+    m.e.points = v->mesh_positions.get();
+    m.e.normals = v->mesh_normals.get();
+    m.e.colors = v->with_color ? v->mesh_colors.get() : nullptr;
+    m.tlimit = tris;
+    m.triangles = v->mesh_triangles.get();
+    O3DB_CUDA_CHECK(launch_pdl_ex(extract_emit_kernel, {grid, kET}, st, m.e));
+    O3DB_CUDA_CHECK(launch_pdl_ex(mesh_triangle_kernel, {grid, kET}, st, m));
     return O3DB_OK;
 }
 
@@ -392,6 +662,94 @@ int o3db_vbg_extract_point_cloud(o3db_vbg* v, float weight_threshold, int64_t ma
         *points = v->ext_points.get();
         *normals = v->ext_normals.get();
         *colors = v->with_color ? v->ext_colors.get() : nullptr;
+    }
+    return O3DB_OK;
+}
+
+int o3db_vbg_extract_triangle_mesh(o3db_vbg* v, float weight_threshold, int64_t estimated_vertex_number,
+                                   int64_t* num_vertices, int64_t* num_triangles, float** vertices, float** normals,
+                                   float** colors, int32_t** triangles, void* stream) {
+    O3DB_REQUIRE(v != nullptr, "o3db_vbg_extract_triangle_mesh: null voxel grid");
+    O3DB_REQUIRE(num_vertices && num_triangles && vertices && normals && colors && triangles,
+                 "o3db_vbg_extract_triangle_mesh: null output");
+    *num_vertices = *num_triangles = 0;
+    *vertices = *normals = *colors = nullptr;
+    *triangles = nullptr;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = ensure_mesh_scratch(v, st);
+    if (rc) return rc;
+    if (estimated_vertex_number > 0) {   // a sizing hint: room for that many vertices and twice as many triangles
+        const int64_t hint = std::min<int64_t>(estimated_vertex_number, INT_MAX);
+        rc = ensure_mesh_rows(v, hint, std::min<int64_t>(2 * hint, INT_MAX), st);
+        if (rc) return rc;
+    }
+    MeshArgs m{};
+    ExtractArgs& a = m.e;
+    a.tab = Table{v->map.table.get(), v->map.nbuckets - 1, v->map.keys.get()};
+    a.size = &v->status->size;
+    a.capacity = (int)v->map.capacity;
+    a.res = v->resolution;
+    a.res3 = v->resolution * v->resolution * v->resolution;
+    a.words = (int)ceil_div(a.res3, 32);
+    a.div_res = fast_div_multiplier((unsigned)a.res);
+    a.div_res2 = fast_div_multiplier((unsigned)(a.res * a.res));
+    a.voxel_size = v->voxel_size;
+    a.weight_threshold = weight_threshold;
+    a.tsdf = v->map.tsdf.get();
+    a.weight = v->map.weight.get();
+    a.color = v->with_color ? v->map.color.get() : nullptr;
+    a.nb = v->mesh_nb.get();
+    a.counts = v->mesh_vcounts.get();
+    a.masks = v->mesh_masks.get();
+    a.total = v->mesh_totals.get();
+    m.cases = v->mesh_cases.get();
+    m.wbase = v->mesh_wbase.get();
+    m.tcounts = v->mesh_tcounts.get();
+    m.ttotal = v->mesh_totals.get() + 1;
+    const unsigned grid = (unsigned)std::min<int64_t>(v->map.capacity, (int64_t)num_sms() * 8);
+    const size_t halo = (size_t)(a.res + 1) * (a.res + 1) * (a.res + 1);   // bytes of the staged voxels or cubes
+    O3DB_CUDA_CHECK(cudaMemsetAsync(v->mesh_totals.get(), 0, 2 * sizeof(unsigned long long), st));
+    extract_neighbors_kernel<<<(unsigned)std::min<int64_t>(ceil_div(v->map.capacity * 27, kET), (int64_t)num_sms() * 8), kET,
+                               0, st>>>(a);
+    O3DB_LAUNCH_CHECK();
+    O3DB_CUDA_CHECK(launch_pdl_ex(mesh_classify_kernel, {grid, kET, halo}, st, m));
+    O3DB_CUDA_CHECK(launch_pdl_ex(mesh_count_kernel, {grid, kET, halo}, st, m));
+    rc = exclusive_scan_u32(v->mesh_vcounts.get(), v->map.capacity, v->mesh_scan.get(), st);
+    if (rc) return rc;
+    rc = exclusive_scan_u32(v->mesh_tcounts.get(), v->map.capacity, v->mesh_scan.get(), st);
+    if (rc) return rc;
+    // emitted before the read-back when the buffers already hold rows (every call but the ones that grow them)
+    const bool ahead = v->mesh_vrows > 0 && v->mesh_trows > 0;
+    const long long ahead_v = ahead ? v->mesh_vrows : 0, ahead_t = ahead ? v->mesh_trows : 0;
+    if (ahead) {
+        rc = launch_mesh_emit(v, m, ahead_v, ahead_t, grid, st);
+        if (rc) return rc;
+    }
+    // the one host synchronisation (read_status's): the two counts and the map status (a frame dropped for capacity)
+    O3DB_CUDA_CHECK(cudaMemcpyAsync(v->h_mesh_totals.get(), v->mesh_totals.get(), 2 * sizeof(long long),
+                                    cudaMemcpyDeviceToHost, st));
+    rc = read_status(v, st);
+    if (rc) return rc;
+    const long long verts = v->h_mesh_totals[0], tris = v->h_mesh_totals[1];
+    if (verts > INT_MAX || tris > INT_MAX) {
+        set_last_error("o3db_vbg_extract_triangle_mesh: the surface has %lld vertices and %lld triangles, more than "
+                       "the %d that Int32 indices can address; raise weight_threshold or extract a smaller volume",
+                       verts, tris, INT_MAX);
+        return O3DB_ERR_INVALID;
+    }
+    if (verts > ahead_v || tris > ahead_t) {
+        rc = ensure_mesh_rows(v, verts, tris, st);
+        if (rc) return rc;
+        rc = launch_mesh_emit(v, m, verts, tris, grid, st);
+        if (rc) return rc;
+    }
+    *num_vertices = verts;
+    *num_triangles = tris;
+    if (verts > 0) {
+        *vertices = v->mesh_positions.get();
+        *normals = v->mesh_normals.get();
+        *colors = v->with_color ? v->mesh_colors.get() : nullptr;
+        *triangles = v->mesh_triangles.get();
     }
     return O3DB_OK;
 }

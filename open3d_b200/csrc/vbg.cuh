@@ -164,6 +164,23 @@ struct o3db_vbg {
     o3db::GridPtr<float> ext_points;
     o3db::GridPtr<float> ext_normals;
     o3db::GridPtr<float> ext_colors;
+    // o3db_vbg_extract_triangle_mesh (extract.cu): its own scratch for mesh_blocks slots and outputs for mesh_vrows
+    // vertices and mesh_trows triangles, so that neither extraction invalidates the other's results
+    int64_t mesh_blocks = 0;
+    o3db::GridPtr<int> mesh_nb;                     // [mesh_blocks][27] neighbour slots, -1 = absent
+    o3db::GridPtr<unsigned char> mesh_cases;        // [mesh_blocks][res^3] cube case, 0 for a cube that does not contribute
+    o3db::GridPtr<unsigned> mesh_vcounts;           // [mesh_blocks + 1] vertices per block, then their exclusive scan
+    o3db::GridPtr<unsigned> mesh_tcounts;           // [mesh_blocks + 1] triangles per block, then their exclusive scan
+    o3db::GridPtr<unsigned> mesh_scan;              // scan tile sums
+    o3db::GridPtr<unsigned> mesh_masks;             // [mesh_blocks][ceil(res^3 / 32)][3] vertex bits per axis
+    o3db::GridPtr<unsigned> mesh_wbase;             // [mesh_blocks][ceil(res^3 / 32)] block's vertices before each word
+    o3db::GridPtr<unsigned long long> mesh_totals;  // 64-bit vertex and triangle counts
+    o3db::PinnedPtr<long long[]> h_mesh_totals;     // pinned read-back of them
+    int64_t mesh_vrows = 0, mesh_trows = 0;
+    o3db::GridPtr<float> mesh_positions;
+    o3db::GridPtr<float> mesh_normals;
+    o3db::GridPtr<float> mesh_colors;
+    o3db::GridPtr<int> mesh_triangles;
 };
 
 namespace o3db {

@@ -537,6 +537,15 @@ class PointCloud:
         return self
 
 
+class TriangleMesh:
+    """t::geometry::TriangleMesh as the TSDF extraction returns it: device tensors in ``vertex`` ("positions",
+    "normals", "colors") and ``triangle`` ("indices", [T, 3] Int32), as upstream's attribute maps."""
+
+    def __init__(self):
+        self.vertex = {}
+        self.triangle = {}
+
+
 class Image:
     """t::geometry::Image as a thin holder of an [H,W,C] tensor."""
 
@@ -904,6 +913,27 @@ class VoxelBlockGrid:
         out.point["normals"] = _s.device_view(nrm.value, (rows, 3), torch.float32).clone()
         if self._with_color:
             out.point["colors"] = _s.device_view(col.value, (rows, 3), torch.float32).clone()
+        return out
+
+    def extract_triangle_mesh(self, weight_threshold=3.0, estimated_vertex_number=-1):
+        """VoxelBlockGrid::ExtractTriangleMesh (VoxelBlockGrid.cpp:436-472; pybind voxel_block_grid.cpp:185-188):
+        marching cubes over the cubes whose 8 voxels all have weight > weight_threshold, as a TriangleMesh with
+        vertex "positions", "normals", "colors" (grids with colour) and triangle "indices".  Vertices in
+        extract_point_cloud's order, triangles by block, voxel and case table (see o3db_vbg_extract_triangle_mesh).
+        estimated_vertex_number only sizes buffers: the mesh is always complete."""
+        nv, nt = C.c_int64(0), C.c_int64(0)
+        pts, nrm, col, tri = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        self._replay.guard(lambda: check(lib.o3db_vbg_extract_triangle_mesh(
+            self._h, float(weight_threshold), int(estimated_vertex_number), C.byref(nv), C.byref(nt), C.byref(pts),
+            C.byref(nrm), C.byref(col), C.byref(tri), current_stream_ptr())))
+        verts, tris = int(nv.value), int(nt.value)
+        # the library's buffers are reused by the next call: copy out
+        out = TriangleMesh()
+        out.vertex["positions"] = _s.device_view(pts.value, (verts, 3), torch.float32).clone()
+        out.vertex["normals"] = _s.device_view(nrm.value, (verts, 3), torch.float32).clone()
+        if self._with_color:
+            out.vertex["colors"] = _s.device_view(col.value, (verts, 3), torch.float32).clone()
+        out.triangle["indices"] = _s.device_view(tri.value, (tris, 3), torch.int32).clone()
         return out
 
     def last_frustum_block_coordinates(self):

@@ -118,6 +118,10 @@ class Model:
         """Model::ExtractPointCloud (slam/Model.cpp:108-111; pybind slam.cpp:112-115)."""
         return self.voxel_grid.extract_point_cloud(weight_threshold, estimated_number)
 
+    def extract_trianglemesh(self, weight_threshold=3.0, estimated_number=-1):
+        """Model::ExtractTriangleMesh (slam/Model.cpp; pybind slam.cpp:119-122)."""
+        return self.voxel_grid.extract_triangle_mesh(weight_threshold, estimated_number)
+
     def track_frame_to_model(self, input_frame, model_frame, depth_scale=1000.0, depth_max=3.0, depth_diff=0.07,
                              method=None, criteria=(6, 3, 1)):
         """Model::TrackFrameToModel (slam/Model.cpp:68-89): multi-scale RGB-D odometry of the input frame against
