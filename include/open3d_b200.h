@@ -14,6 +14,10 @@
  *  - `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).
  *    Calls are asynchronous on `stream` unless they return values to the host,
  *    in which case they synchronise that stream (never the device).
+ *  - A handle (o3db_knn, o3db_nns, o3db_icp) may be used on another stream than the one it was created on: the
+ *    call first waits for the work queued on the creation stream so far (the creation included), and the creation
+ *    stream, on which destroy frees the handle's buffers, is ordered after the call.  Nothing of this is done for a
+ *    call on the creation stream.  The thread-safety rule below holds here too: no two calls on one handle at once.
  *  - Return value: O3DB_OK (0) or a negative o3db_status; o3db_last_error()
  *    returns a thread-local message.  There is NO CPU fallback: without a CUDA
  *    device every compute entry point fails with O3DB_ERR_CUDA.

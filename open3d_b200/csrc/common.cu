@@ -47,6 +47,36 @@ void configure_memory_pool() {
     configured_device = dev;
 }
 
+HandleEvents::~HandleEvents() {
+    if (ready) cudaEventDestroy(ready);
+    if (used) cudaEventDestroy(used);
+}
+
+static cudaError_t wait_for_home(const HandleEvents& e, cudaStream_t home, cudaStream_t st) {
+    cudaError_t err = cudaSuccess;
+    if (!e.ready && (err = cudaEventCreateWithFlags(&e.ready, cudaEventDisableTiming)) != cudaSuccess) return err;
+    if (!e.used && (err = cudaEventCreateWithFlags(&e.used, cudaEventDisableTiming)) != cudaSuccess) return err;
+    if ((err = cudaEventRecord(e.ready, home)) != cudaSuccess) return err;
+    return cudaStreamWaitEvent(st, e.ready, 0);
+}
+
+HandleUse::HandleUse(const HandleEvents& e, cudaStream_t home, cudaStream_t st) : e_(e), home_(home), st_(st) {
+    if (st_ == home_) return;
+    const cudaError_t err = wait_for_home(e_, home_, st_);
+    if (err != cudaSuccess) {
+        (void)cudaGetLastError();
+        set_last_error("ordering the call after the handle's creation stream failed: %s", cudaGetErrorString(err));
+        status_ = O3DB_ERR_CUDA;
+        st_ = home_;   // nothing was ordered after the wait, so there is nothing to order home after either
+    }
+}
+
+HandleUse::~HandleUse() {
+    if (st_ == home_) return;
+    // (a handle's destroy ignores errors too: there is no caller left to report them to)
+    if (cudaEventRecord(e_.used, st_) == cudaSuccess) cudaStreamWaitEvent(home_, e_.used, 0);
+}
+
 static std::mutex g_pinned_mu;
 static std::vector<void*> g_pinned_free;
 

@@ -150,6 +150,37 @@ struct HandleDestroy {
     void operator()(H* h) const { Destroy(h); }
 };
 
+// Cross-stream order of a handle that outlives its create call (o3db_knn, o3db_nns, o3db_icp).  Its buffers are
+// allocated on the creation stream ("home"), and its destroy drains that stream and frees them on it.  A call may use
+// the handle on another stream: it then records `ready` on home and waits on it, so that it runs after everything
+// queued on home so far (the tail of create included), and afterwards records `used` on its own stream and makes home
+// wait on that, so that home, and with it destroy's frees, come after every use.  The two events are created on the
+// first such call; on the creation stream none of this is needed and nothing is done.  One call at a time per handle
+// (the header's one-handle-per-host-thread rule): the events are shared by the handle's calls.
+struct HandleEvents {
+    mutable cudaEvent_t ready = nullptr;
+    mutable cudaEvent_t used = nullptr;
+    HandleEvents() = default;
+    HandleEvents(const HandleEvents&) = delete;
+    HandleEvents& operator=(const HandleEvents&) = delete;
+    ~HandleEvents();
+};
+// Scope of one call on a handle: the wait on home when st is not home (check status()), and on every way out of the
+// scope the `used` record that orders home after st.
+class HandleUse {
+  public:
+    HandleUse(const HandleEvents& e, cudaStream_t home, cudaStream_t st);
+    ~HandleUse();
+    int status() const { return status_; }
+    HandleUse(const HandleUse&) = delete;
+    HandleUse& operator=(const HandleUse&) = delete;
+
+  private:
+    const HandleEvents& e_;
+    cudaStream_t home_, st_;
+    int status_ = O3DB_OK;
+};
+
 #ifdef __CUDACC__
 // Programmatic dependent launch: a kernel launched through launch_pdl_ex may become resident while its predecessor
 // on the stream drains; it must call pdl_wait() before touching anything the predecessor wrote.

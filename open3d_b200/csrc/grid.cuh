@@ -38,6 +38,7 @@ struct Grid {
 // o3db_knn, the k-nearest-neighbour index.
 struct o3db_nns {
     cudaStream_t stream = 0;   // creation stream (buffers are freed on it)
+    o3db::HandleEvents events;   // use on other streams (the public handles: o3db_nns, o3db_knn, o3db_icp)
     o3db::Grid g{};
     double radius = 0;
     int64_t m = 0;

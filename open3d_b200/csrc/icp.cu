@@ -2074,7 +2074,8 @@ int o3db_nns_create(const float* points_dev, int64_t num_points, double radius, 
 
 void o3db_nns_destroy(o3db_nns* nns) {
     if (!nns) return;
-    cudaStreamSynchronize(nns->stream);   // searches may still be in flight on the creation stream
+    // searches may still be in flight on the creation stream, and it waits for those on other streams
+    cudaStreamSynchronize(nns->stream);
     delete nns;
 }
 
@@ -2091,6 +2092,8 @@ int o3db_nns_hybrid_search(const o3db_nns* nns, const float* queries_dev, int64_
     const float thr = r * r, rr = r * (1.0f + 1e-6f);
     const unsigned nb = (unsigned)ceil_div(num_queries, kThreads);
     cudaStream_t st = (cudaStream_t)stream;
+    const HandleUse use(nns->events, nns->stream, st);
+    if (use.status()) return use.status();
     if (max_knn == 1)
         hybrid_search_k1_kernel<true><<<nb, kThreads, 0, st>>>(nns->g, nns->pts4.get(), nns->cell_start.get(), queries_dev,
                                                                num_queries, rr, thr, indices_dev, distances_dev,
@@ -2555,8 +2558,9 @@ int o3db_get_information_matrix(const float* source_dev, int64_t n, const float*
 
 void o3db_icp_destroy(o3db_icp* c) {
     if (!c) return;
-    // Every buffer was allocated, and all work on it enqueued, on the handle's stream: drain it (the pinned block
-    // may still be the target of a D2H copy); the owners then free in stream order on the same stream.
+    // Every buffer was allocated on the handle's stream, and work enqueued on other streams is ordered before its
+    // later work (HandleUse): drain it (the pinned block may still be the target of a D2H copy); the owners then free
+    // in stream order on the same stream.
     cudaStreamSynchronize(c->stream);
     delete c;
 }
@@ -2786,6 +2790,8 @@ int o3db_icp_create_doppler(const float* source_dev, const float* source_doppler
 int o3db_icp_reset(o3db_icp* c, void* stream) {
     O3DB_REQUIRE(c != nullptr, "o3db_icp_reset: null handle");
     cudaStream_t st = (cudaStream_t)stream;
+    const HandleUse use(c->nns.events, c->stream, st);
+    if (use.status()) return use.status();
     int rc = icp_gather_source(c, st);
     if (rc) return rc;
     return icp_init_state(c, st);
@@ -2794,6 +2800,8 @@ int o3db_icp_reset(o3db_icp* c, void* stream) {
 int o3db_icp_iterate(o3db_icp* c, int iterations, void* stream) {
     O3DB_REQUIRE(c != nullptr, "o3db_icp_iterate: null handle");
     cudaStream_t st = (cudaStream_t)stream;
+    const HandleUse use(c->nns.events, c->stream, st);
+    if (use.status()) return use.status();
     const int todo = std::min(iterations, c->opt.max_iteration - c->launched);
     IcpArgs a = make_args(c);
     for (int k = 0; k < todo; ++k) {
@@ -2841,6 +2849,8 @@ int o3db_icp_finish(o3db_icp* c, o3db_icp_result* result, int64_t* correspondenc
                     void* stream) {
     O3DB_REQUIRE(c != nullptr && result != nullptr, "o3db_icp_finish: null argument");
     cudaStream_t st = (cudaStream_t)stream;
+    const HandleUse use(c->nns.events, c->stream, st);
+    if (use.status()) return use.status();
     IcpArgs a = make_args(c);
     a.corr_out = correspondences_dev;
     O3DB_CUDA_CHECK(launch_icp(c, 1, st, a));
@@ -2855,6 +2865,8 @@ int o3db_icp_finish(o3db_icp* c, o3db_icp_result* result, int64_t* correspondenc
 
 int o3db_icp_state(o3db_icp* c, o3db_icp_result* result, double* per_iteration_host, void* stream) {
     O3DB_REQUIRE(c != nullptr && result != nullptr, "o3db_icp_state: null argument");
+    const HandleUse use(c->nns.events, c->stream, (cudaStream_t)stream);
+    if (use.status()) return use.status();
     return icp_read_state(c, result, per_iteration_host, (cudaStream_t)stream);
 }
 

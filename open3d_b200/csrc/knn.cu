@@ -637,7 +637,8 @@ int o3db_knn_create(const float* points_dev, int64_t num_points, void* stream, o
 
 void o3db_knn_destroy(o3db_knn* knn) {
     if (!knn) return;
-    cudaStreamSynchronize(knn->grid.stream);   // searches may still be in flight on the creation stream
+    // searches may still be in flight on the creation stream, and it waits for those on other streams
+    cudaStreamSynchronize(knn->grid.stream);
     delete knn;
 }
 
@@ -662,6 +663,8 @@ int o3db_knn_search(const o3db_knn* knn, const float* queries_dev, int64_t num_q
     const int kp = (int)std::min<int64_t>(knn_k, knn->grid.m);
     const unsigned nb = (unsigned)ceil_div(num_queries, kThreads / 32);
     cudaStream_t st = (cudaStream_t)stream;
+    const HandleUse use(knn->grid.events, knn->grid.stream, st);
+    if (use.status()) return use.status();
     if (index_dtype == O3DB_INDEX_INT32)
         knn_search_kernel<int32_t><<<nb, kThreads, 0, st>>>(knn_view(knn), queries_dev, num_queries, kp,
                                                             static_cast<int32_t*>(indices_dev), distances_dev);
@@ -682,6 +685,8 @@ int o3db_knn_search_lists(const o3db_knn* knn, const float* queries_dev, int64_t
     if (num_queries == 0) return O3DB_OK;
     O3DB_REQUIRE(queries_dev && indices_dev && distances_dev && counts_dev, "o3db_knn_search_lists: null argument");
     cudaStream_t st = (cudaStream_t)stream;
+    const HandleUse use(knn->grid.events, knn->grid.stream, st);
+    if (use.status()) return use.status();
     DevPtr<unsigned> bad;
     if (int rc = dev_alloc(bad, 1, st)) return rc;
     O3DB_CUDA_CHECK(cudaMemsetAsync(bad.get(), 0, sizeof(unsigned), st));
