@@ -291,6 +291,32 @@ inline RegistrationResult ToRegistrationResult(const o3db_icp_result& r, const s
     return out;
 }
 
+namespace detail {
+/// What every registration::ICP overload does after its estimator's own checks: the distance and voxel checks (the
+/// overload's own voxel message), the options (kernel null: opt.kernel stays zeroed), the per-iteration buffer, the C
+/// call run(options, result, per_iteration) and the result.
+template <class Run>
+inline RegistrationResult RunICP(double max_correspondence_distance, double voxel_size, const char* voxel_message,
+                                 const ICPConvergenceCriteria& criteria, const RobustKernel* kernel,
+                                 const IterationCallback& callback_after_iteration, int64_t* correspondences_dev,
+                                 const Run& run) {
+    if (max_correspondence_distance <= 0.0)
+        throw std::runtime_error(" Max correspondence distance must be greater than 0, but got " +
+                                 std::to_string(max_correspondence_distance) + " in scale: 0.");
+    if (voxel_size > 0) throw std::runtime_error(voxel_message);
+    o3db_icp_options opt{};
+    opt.max_correspondence_distance = max_correspondence_distance;
+    opt.max_iteration = criteria.max_iteration_;
+    opt.relative_fitness = criteria.relative_fitness_;
+    opt.relative_rmse = criteria.relative_rmse_;
+    if (kernel) opt.kernel = {static_cast<int>(kernel->type_), kernel->scaling_parameter_, kernel->shape_parameter_};
+    o3db_icp_result r{};
+    std::vector<double> per(2 * static_cast<size_t>(criteria.max_iteration_ > 0 ? criteria.max_iteration_ : 1), 0.0);
+    Check(run(&opt, &r, per.data()));
+    return ToRegistrationResult(r, per, correspondences_dev, callback_after_iteration);
+}
+}  // namespace detail
+
 /// registration::ICP (Registration.h:133-144, Registration.cpp:93-106) for
 /// TransformationEstimationPointToPlane; voxel_size must be <= 0 here (down-sample with
 /// o3db_voxel_down_sample beforehand; the Python surface builds the pyramid itself).
@@ -306,23 +332,15 @@ inline RegistrationResult ICP(const geometry::PointCloud& source, const geometry
         throw std::runtime_error("Source and/or Target pointcloud is empty.");
     if (!target.HasPointNormals())
         throw std::runtime_error("TransformationEstimationPointToPlane require pre-computed normal vectors for target PointCloud.");
-    if (max_correspondence_distance <= 0.0)
-        throw std::runtime_error(" Max correspondence distance must be greater than 0, but got " +
-                                 std::to_string(max_correspondence_distance) + " in scale: 0.");
-    if (voxel_size > 0)
-        throw std::runtime_error("voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample); this header-only wrapper owns no device memory for the pyramid");
-    o3db_icp_options opt{};
-    opt.max_correspondence_distance = max_correspondence_distance;
-    opt.max_iteration = criteria.max_iteration_;
-    opt.relative_fitness = criteria.relative_fitness_;
-    opt.relative_rmse = criteria.relative_rmse_;
-    opt.kernel = {static_cast<int>(estimation.kernel_.type_), estimation.kernel_.scaling_parameter_,
-                  estimation.kernel_.shape_parameter_};
-    o3db_icp_result r{};
-    std::vector<double> per(2 * static_cast<size_t>(criteria.max_iteration_ > 0 ? criteria.max_iteration_ : 1), 0.0);
-    Check(o3db_icp_point_to_plane(source.positions, source.num_points, target.positions, target.normals, target.num_points,
-                                  init_source_to_target.data(), &opt, &r, correspondences_dev, per.data(), stream));
-    return ToRegistrationResult(r, per, correspondences_dev, callback_after_iteration);
+    return detail::RunICP(
+            max_correspondence_distance, voxel_size,
+            "voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample); this header-only wrapper owns no device memory for the pyramid",
+            criteria, &estimation.kernel_, callback_after_iteration, correspondences_dev,
+            [&](const o3db_icp_options* opt, o3db_icp_result* r, double* per) {
+                return o3db_icp_point_to_plane(source.positions, source.num_points, target.positions, target.normals,
+                                               target.num_points, init_source_to_target.data(), opt, r, correspondences_dev,
+                                               per, stream);
+            });
 }
 
 /// registration::ICP for TransformationEstimationForColoredICP.  The target needs color_gradients
@@ -340,24 +358,16 @@ inline RegistrationResult ICP(const geometry::PointCloud& source, const geometry
     if (!target.HasPointColors()) throw std::runtime_error("ColoredICP requires target pointcloud to have colors.");
     if (!source.HasPointColors()) throw std::runtime_error("ColoredICP requires source pointcloud to have colors.");
     if (!target.color_gradients) throw std::runtime_error("Target pointcloud missing color_gradients attribute.");
-    if (max_correspondence_distance <= 0.0)
-        throw std::runtime_error(" Max correspondence distance must be greater than 0, but got " +
-                                 std::to_string(max_correspondence_distance) + " in scale: 0.");
-    if (voxel_size > 0)
-        throw std::runtime_error("voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample_attrs)");
-    o3db_icp_options opt{};
-    opt.max_correspondence_distance = max_correspondence_distance;
-    opt.max_iteration = criteria.max_iteration_;
-    opt.relative_fitness = criteria.relative_fitness_;
-    opt.relative_rmse = criteria.relative_rmse_;
-    opt.kernel = {static_cast<int>(estimation.kernel_.type_), estimation.kernel_.scaling_parameter_,
-                  estimation.kernel_.shape_parameter_};
-    o3db_icp_result r{};
-    std::vector<double> per(2 * static_cast<size_t>(criteria.max_iteration_ > 0 ? criteria.max_iteration_ : 1), 0.0);
-    Check(o3db_icp_colored(source.positions, source.colors, source.num_points, target.positions, target.normals,
-                           target.colors, target.color_gradients, target.num_points, init_source_to_target.data(), &opt,
-                           estimation.lambda_geometric_, &r, correspondences_dev, per.data(), stream));
-    return ToRegistrationResult(r, per, correspondences_dev, callback_after_iteration);
+    return detail::RunICP(
+            max_correspondence_distance, voxel_size,
+            "voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample_attrs)", criteria,
+            &estimation.kernel_, callback_after_iteration, correspondences_dev,
+            [&](const o3db_icp_options* opt, o3db_icp_result* r, double* per) {
+                return o3db_icp_colored(source.positions, source.colors, source.num_points, target.positions,
+                                        target.normals, target.colors, target.color_gradients, target.num_points,
+                                        init_source_to_target.data(), opt, estimation.lambda_geometric_, r,
+                                        correspondences_dev, per, stream);
+            });
 }
 
 /// registration::ICP for TransformationEstimationPointToPoint (upstream's default estimator, Registration.h:140):
@@ -370,21 +380,14 @@ inline RegistrationResult ICP(const geometry::PointCloud& source, const geometry
                               int64_t* correspondences_dev = nullptr, void* stream = nullptr) {
     if (!target.HasPointPositions() || !source.HasPointPositions())
         throw std::runtime_error("Source and/or Target pointcloud is empty.");
-    if (max_correspondence_distance <= 0.0)
-        throw std::runtime_error(" Max correspondence distance must be greater than 0, but got " +
-                                 std::to_string(max_correspondence_distance) + " in scale: 0.");
-    if (voxel_size > 0)
-        throw std::runtime_error("voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample)");
-    o3db_icp_options opt{};
-    opt.max_correspondence_distance = max_correspondence_distance;
-    opt.max_iteration = criteria.max_iteration_;
-    opt.relative_fitness = criteria.relative_fitness_;
-    opt.relative_rmse = criteria.relative_rmse_;
-    o3db_icp_result r{};
-    std::vector<double> per(2 * static_cast<size_t>(criteria.max_iteration_ > 0 ? criteria.max_iteration_ : 1), 0.0);
-    Check(o3db_icp_point_to_point(source.positions, source.num_points, target.positions, target.num_points,
-                                  init_source_to_target.data(), &opt, &r, correspondences_dev, per.data(), stream));
-    return ToRegistrationResult(r, per, correspondences_dev, callback_after_iteration);
+    return detail::RunICP(max_correspondence_distance, voxel_size,
+                          "voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample)", criteria,
+                          nullptr, callback_after_iteration, correspondences_dev,
+                          [&](const o3db_icp_options* opt, o3db_icp_result* r, double* per) {
+                              return o3db_icp_point_to_point(source.positions, source.num_points, target.positions,
+                                                             target.num_points, init_source_to_target.data(), opt, r,
+                                                             correspondences_dev, per, stream);
+                          });
 }
 
 /// registration::ICP for TransformationEstimationSymmetric (and registration_symmetric_icp, Registration.cpp:108-117):
@@ -399,24 +402,15 @@ inline RegistrationResult ICP(const geometry::PointCloud& source, const geometry
         throw std::runtime_error("Source and/or Target pointcloud is empty.");
     if (!source.HasPointNormals() || !target.HasPointNormals())
         throw std::runtime_error("SymmetricICP requires both source and target pointclouds to have normals.");
-    if (max_correspondence_distance <= 0.0)
-        throw std::runtime_error(" Max correspondence distance must be greater than 0, but got " +
-                                 std::to_string(max_correspondence_distance) + " in scale: 0.");
-    if (voxel_size > 0)
-        throw std::runtime_error("voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample)");
-    o3db_icp_options opt{};
-    opt.max_correspondence_distance = max_correspondence_distance;
-    opt.max_iteration = criteria.max_iteration_;
-    opt.relative_fitness = criteria.relative_fitness_;
-    opt.relative_rmse = criteria.relative_rmse_;
-    opt.kernel = {static_cast<int>(estimation.kernel_.type_), estimation.kernel_.scaling_parameter_,
-                  estimation.kernel_.shape_parameter_};
-    o3db_icp_result r{};
-    std::vector<double> per(2 * static_cast<size_t>(criteria.max_iteration_ > 0 ? criteria.max_iteration_ : 1), 0.0);
-    Check(o3db_icp_symmetric(source.positions, source.normals, source.num_points, target.positions, target.normals,
-                             target.num_points, init_source_to_target.data(), &opt, &r, correspondences_dev, per.data(),
-                             stream));
-    return ToRegistrationResult(r, per, correspondences_dev, callback_after_iteration);
+    return detail::RunICP(max_correspondence_distance, voxel_size,
+                          "voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample)", criteria,
+                          &estimation.kernel_, callback_after_iteration, correspondences_dev,
+                          [&](const o3db_icp_options* opt, o3db_icp_result* r, double* per) {
+                              return o3db_icp_symmetric(source.positions, source.normals, source.num_points,
+                                                        target.positions, target.normals, target.num_points,
+                                                        init_source_to_target.data(), opt, r, correspondences_dev, per,
+                                                        stream);
+                          });
 }
 
 /// registration::ICP for TransformationEstimationForDopplerICP: the source needs dopplers and directions (never
@@ -434,23 +428,16 @@ inline RegistrationResult ICP(const geometry::PointCloud& source, const geometry
         throw std::runtime_error("DopplerICP requires source pointcloud to have Doppler velocities.");
     if (source.directions == nullptr)
         throw std::runtime_error("DopplerICP requires source pointcloud to have pre-computed direction vectors.");
-    if (max_correspondence_distance <= 0.0)
-        throw std::runtime_error(" Max correspondence distance must be greater than 0, but got " +
-                                 std::to_string(max_correspondence_distance) + " in scale: 0.");
-    if (voxel_size > 0)
-        throw std::runtime_error("voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample)");
-    o3db_icp_options opt{};
-    opt.max_correspondence_distance = max_correspondence_distance;
-    opt.max_iteration = criteria.max_iteration_;
-    opt.relative_fitness = criteria.relative_fitness_;
-    opt.relative_rmse = criteria.relative_rmse_;
     const o3db_doppler_params p = estimation.Params();
-    o3db_icp_result r{};
-    std::vector<double> per(2 * static_cast<size_t>(criteria.max_iteration_ > 0 ? criteria.max_iteration_ : 1), 0.0);
-    Check(o3db_icp_doppler(source.positions, source.dopplers, source.directions, source.num_points, target.positions,
-                           target.normals, target.num_points, init_source_to_target.data(), &opt, &p, &r,
-                           correspondences_dev, per.data(), stream));
-    return ToRegistrationResult(r, per, correspondences_dev, callback_after_iteration);
+    return detail::RunICP(max_correspondence_distance, voxel_size,
+                          "voxel_size > 0: apply PointCloud::VoxelDownSample first (o3db_voxel_down_sample)", criteria,
+                          nullptr, callback_after_iteration, correspondences_dev,
+                          [&](const o3db_icp_options* opt, o3db_icp_result* r, double* per) {
+                              return o3db_icp_doppler(source.positions, source.dopplers, source.directions,
+                                                      source.num_points, target.positions, target.normals,
+                                                      target.num_points, init_source_to_target.data(), opt, &p, r,
+                                                      correspondences_dev, per, stream);
+                          });
 }
 
 /// registration::GetInformationMatrix (Registration.cpp:446-485): row-major 6x6 Float64 GTG on the host.

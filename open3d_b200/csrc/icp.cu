@@ -1908,25 +1908,20 @@ struct o3db_icp {
     o3db::PinnedPtr<IcpState> h_st;
     o3db_comm* comm = nullptr;
     int grid_blocks = 0;
-    int64_t src_keys = 0;            // size of the source sort key space
     int launched = 0;
+    int est = o3db::kEstPlane;       // the estimator (kEst*): the kernels, source record and stage the handle uses
     bool l2loss = true;
     // ColoredICP (TransformationEstimationForColoredICP); null / unused for point-to-plane
-    bool colored = false;
-    const float* src_colors_user = nullptr;
     o3db::DevPtr<float4> tcg4;       // sorted target: colour gradient xyz + intensity
     o3db::DevPtr<float> sint;        // sorted source: intensity
     double lambda_geometric = 0.968;
     // TransformationEstimationPointToPoint: no target normals (nns.nrm4 stays null), no robust kernel
-    bool point = false;
     float pivot[3] = {0.f, 0.f, 0.f};
     // TransformationEstimationSymmetric: 8-plane records carrying the source normals, and the second sum line
-    bool symmetric = false;
     const float* src_normals_user = nullptr;
     o3db::DevPtr<float> chunk_sums2;    // n_pad / 4 floats: 8 per 32-query chunk
     o3db::DevPtr<double> partials2;     // grid_blocks x 8
     // TransformationEstimationForDopplerICP: 9-plane records carrying the source directions and Doppler values
-    bool doppler = false;
     const float* src_dopplers_user = nullptr;
     const float* src_directions_user = nullptr;
     o3db::DopplerConst dop{};
@@ -1934,33 +1929,52 @@ struct o3db_icp {
 
 namespace o3db {
 
-typedef void (*IcpKernel)(IcpArgs);
-// mode 0 = iterate (loss / colour of the handle), 1 = final evaluation (no Jacobian)
-static IcpKernel icp_kernel_for(const o3db_icp* c, int mode) {
-    if (c->doppler)
-        return mode == 1 ? icp_doppler_iteration_kernel<true, 1>
-                         : c->l2loss ? icp_doppler_iteration_kernel<true, 0> : icp_doppler_iteration_kernel<false, 0>;
-    if (c->symmetric)
-        return mode == 1 ? icp_symmetric_iteration_kernel<true, 1>
-                         : c->l2loss ? icp_symmetric_iteration_kernel<true, 0> : icp_symmetric_iteration_kernel<false, 0>;
-    if (mode == 1) return icp_iteration_kernel<true, 1, false>;
-    if (c->point) return icp_point_iteration_kernel;
-    if (c->colored) return c->l2loss ? icp_iteration_kernel<true, 0, true> : icp_iteration_kernel<false, 0, true>;
-    return c->l2loss ? icp_iteration_kernel<true, 0, false> : icp_iteration_kernel<false, 0, false>;
+// f(std::integral_constant<int, kEstX>{}) for the runtime estimator est: the one place the host turns a handle's
+// estimator into the compile-time value its kernels, source record (SrcOf) and stage (IcpStagedSmem) are written for
+template <typename F>
+static auto with_estimator(int est, F&& f) {
+    switch (est) {
+    case kEstColored: return f(std::integral_constant<int, kEstColored>{});
+    case kEstPoint: return f(std::integral_constant<int, kEstPoint>{});
+    case kEstSymmetric: return f(std::integral_constant<int, kEstSymmetric>{});
+    case kEstDoppler: return f(std::integral_constant<int, kEstDoppler>{});
+    default: return f(std::integral_constant<int, kEstPlane>{});
+    }
 }
 
-// dynamic shared memory of the handle's iteration kernels (the stage ring)
-static size_t icp_smem_bytes(const o3db_icp* c, int mode) {
-    if (c->symmetric) return sizeof(IcpStagedSmem<kEstSymmetric>);
-    if (c->doppler) return sizeof(IcpStagedSmem<kEstDoppler>);
-    if (mode == 1) return sizeof(IcpStagedSmem<kEstPlane>);
-    return c->colored ? sizeof(IcpStagedSmem<kEstColored>) : c->point ? sizeof(IcpStagedSmem<kEstPoint>) : sizeof(IcpStagedSmem<kEstPlane>);
+typedef void (*IcpKernel)(IcpArgs);
+struct IcpLaunch {   // an iteration kernel and its dynamic shared memory (the stage ring)
+    IcpKernel kernel;
+    size_t smem;
+};
+// mode 0 = iterate (loss / estimator of the handle), 1 = final evaluation (no Jacobian).  The 5-plane records'
+// evaluation pass is the plane kernel's; the symmetric and Doppler records' strides are compile-time constants of their
+// kernels, so those estimators evaluate with their own.
+static IcpLaunch icp_launch_for(const o3db_icp* c, int mode) {
+    return with_estimator(c->est, [&](auto e) -> IcpLaunch {
+        constexpr int E = decltype(e)::value;
+        constexpr size_t smem = sizeof(IcpStagedSmem<E>);
+        if constexpr (E == kEstSymmetric)
+            return {mode == 1 ? icp_symmetric_iteration_kernel<true, 1>
+                    : c->l2loss ? icp_symmetric_iteration_kernel<true, 0> : icp_symmetric_iteration_kernel<false, 0>, smem};
+        else if constexpr (E == kEstDoppler)
+            return {mode == 1 ? icp_doppler_iteration_kernel<true, 1>
+                    : c->l2loss ? icp_doppler_iteration_kernel<true, 0> : icp_doppler_iteration_kernel<false, 0>, smem};
+        else if (mode == 1)
+            return {icp_iteration_kernel<true, 1, false>, sizeof(IcpStagedSmem<kEstPlane>)};
+        else if constexpr (E == kEstPoint)
+            return {icp_point_iteration_kernel, smem};
+        else
+            return {c->l2loss ? icp_iteration_kernel<true, 0, E == kEstColored> : icp_iteration_kernel<false, 0, E == kEstColored>,
+                    smem};
+    });
 }
 
 // The kernel's griddepcontrol.wait orders it after the previous kernel on the stream; everything before that wait
 // may overlap the predecessor's tail.
 static cudaError_t launch_icp(const o3db_icp* c, int mode, cudaStream_t st, const IcpArgs& a) {
-    return launch_pdl_ex(icp_kernel_for(c, mode), {(unsigned)c->grid_blocks, kIcpThreads, icp_smem_bytes(c, mode)}, st, a);
+    const IcpLaunch k = icp_launch_for(c, mode);
+    return launch_pdl_ex(k.kernel, {(unsigned)c->grid_blocks, kIcpThreads, k.smem}, st, a);
 }
 static IcpArgs make_args(o3db_icp* c) {
     IcpArgs a{};
@@ -1997,7 +2011,7 @@ static IcpArgs make_args(o3db_icp* c) {
     a.sint = c->sint.get();
     a.sqrt_lg = (float)sqrt(c->lambda_geometric);          // RegistrationCUDA.cu:205-208
     a.sqrt_lp = (float)sqrt(1.0 - c->lambda_geometric);
-    a.point_to_point = c->point ? 1 : 0;
+    a.point_to_point = c->est == kEstPoint ? 1 : 0;
     for (int k = 0; k < 3; ++k) a.pivot[k] = c->pivot[k];
     a.chunk_sums2 = c->chunk_sums2.get();
     a.partials2 = c->partials2.get();
@@ -2014,15 +2028,11 @@ static int icp_init_state(o3db_icp* c, cudaStream_t st) {
     memcpy(c->h_st.get(), &h, sizeof(h));
     O3DB_CUDA_CHECK(cudaMemcpyAsync(c->st.get(), c->h_st.get(), sizeof(IcpState), cudaMemcpyHostToDevice, st));
     const unsigned nb = (unsigned)ceil_div(c->n_pad, kThreads);
-    if (c->symmetric)
-        src_blocked_init_kernel<<<nb, kThreads, 0, st>>>(SrcBlockedSym{c->src_blk.get()}, c->n, c->n_pad, false);
-    else if (c->doppler)
-        src_blocked_init_kernel<<<nb, kThreads, 0, st>>>(SrcBlockedDop{c->src_blk.get()}, c->n, c->n_pad, false);
-    else
-        src_blocked_init_kernel<<<nb, kThreads, 0, st>>>(SrcBlocked{c->src_blk.get()}, c->n, c->n_pad,
-                                                         false);   // no seeds, no clearances
+    with_estimator(c->est, [&](auto e) {   // no seeds, no clearances
+        src_blocked_init_kernel<<<nb, kThreads, 0, st>>>(SrcOf<decltype(e)::value>{c->src_blk.get()}, c->n, c->n_pad, false);
+    });
     O3DB_LAUNCH_CHECK();
-    if (c->doppler) {   // the first iteration's velocity, on the device like every later one
+    if (c->est == kEstDoppler) {   // the first iteration's velocity, on the device like every later one
         doppler_init_kernel<<<1, 32, 0, st>>>(make_args(c));
         O3DB_LAUNCH_CHECK();
     }
@@ -2035,18 +2045,13 @@ static int icp_gather_source(o3db_icp* c, cudaStream_t st) {
     for (int i = 0; i < 16; ++i) T0.m[i] = (float)c->init_T[i];   // Transform.cpp:29-31: T cast to the point dtype
     if (c->n == 0) return O3DB_OK;
     const unsigned nb = (unsigned)ceil_div(c->n, kThreads);
-    if (c->symmetric)
+    with_estimator(c->est, [&](auto e) {   // (src_normals_user is null but for the symmetric handle, the only reader)
         scatter_source_kernel<<<nb, kThreads, 0, st>>>(c->src_user, c->src_normals_user, c->n, T0, c->src_start.get(),
-                                                       c->src_key.get(), c->src_rank.get(), SrcBlockedSym{c->src_blk.get()},
-                                                       c->src_idx.get());
-    else if (c->doppler)
-        scatter_source_kernel<<<nb, kThreads, 0, st>>>(c->src_user, nullptr, c->n, T0, c->src_start.get(), c->src_key.get(),
-                                                       c->src_rank.get(), SrcBlockedDop{c->src_blk.get()}, c->src_idx.get());
-    else
-        scatter_source_kernel<<<nb, kThreads, 0, st>>>(c->src_user, nullptr, c->n, T0, c->src_start.get(), c->src_key.get(),
-                                                       c->src_rank.get(), SrcBlocked{c->src_blk.get()}, c->src_idx.get());
+                                                       c->src_key.get(), c->src_rank.get(),
+                                                       SrcOf<decltype(e)::value>{c->src_blk.get()}, c->src_idx.get());
+    });
     O3DB_LAUNCH_CHECK();
-    if (c->doppler) {
+    if (c->est == kEstDoppler) {
         scatter_doppler_planes_kernel<<<nb, kThreads, 0, st>>>(c->src_directions_user, c->src_dopplers_user, c->n,
                                                                c->src_idx.get(), SrcBlockedDop{c->src_blk.get()});
         O3DB_LAUNCH_CHECK();
@@ -2568,9 +2573,8 @@ void o3db_icp_destroy(o3db_icp* c) {
 }  // extern "C"
 
 namespace o3db {
-struct EstimatorInputs {   // all device pointers; null source_colors and source_normals and no point_to_point = plain
-                           // point-to-plane
-    bool point_to_point = false;   // no target normals wanted
+struct EstimatorInputs {   // the estimator and the inputs only it reads (device pointers)
+    int est;                                 // kEst*
     const float* source_normals = nullptr;   // symmetric
     const float* source_dopplers = nullptr;   // Doppler (with source_directions and dop)
     const float* source_directions = nullptr;
@@ -2591,7 +2595,7 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     O3DB_REQUIRE(options != nullptr && init_T != nullptr, "o3db_icp_create: null options / init");
     // Registration.cpp:119-219 AssertInputMultiScaleICP
     O3DB_REQUIRE(source_dev && target_dev && n > 0 && m > 0, "Source and/or Target pointcloud is empty.");
-    O3DB_REQUIRE(col.point_to_point || target_normals_dev != nullptr, "Target pointcloud missing normals attribute.");
+    O3DB_REQUIRE(col.est == kEstPoint || target_normals_dev != nullptr, "Target pointcloud missing normals attribute.");
     O3DB_REQUIRE(n < INT_MAX - 2048 && m < INT_MAX - 2048, "o3db_icp_create: too many points");
     O3DB_REQUIRE(options->max_correspondence_distance > 0, "max_correspondence_distance must be positive");
     O3DB_REQUIRE(options->max_iteration >= 0, "max_iteration must be non-negative");
@@ -2603,22 +2607,20 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     c->src_user = source_dev;
     c->n = n;
     c->comm = comm;
-    c->point = col.point_to_point;
-    c->symmetric = col.source_normals != nullptr;
+    c->est = col.est;
     c->src_normals_user = col.source_normals;
-    c->doppler = col.dop != nullptr;
     c->src_dopplers_user = col.source_dopplers;
     c->src_directions_user = col.source_directions;
     if (col.dop) c->dop = *col.dop;
-    c->l2loss = c->point || (col.dop ? col.dop->geo.method == O3DB_ROBUST_L2 && col.dop->dop.method == O3DB_ROBUST_L2
-                                     : options->kernel.method == O3DB_ROBUST_L2);
-    c->colored = col.source_colors != nullptr;
-    c->src_colors_user = col.source_colors;
+    c->l2loss = c->est == kEstPoint ||
+                (c->est == kEstDoppler ? col.dop->geo.method == O3DB_ROBUST_L2 && col.dop->dop.method == O3DB_ROBUST_L2
+                                       : options->kernel.method == O3DB_ROBUST_L2);
     c->lambda_geometric = col.lambda_geometric;
     memcpy(c->init_T, init_T, sizeof(c->init_T));
     // fine cells (half the radius) by default: pass 1 of the two-pass search then covers the
     // +-1 cell box, which holds the nearest neighbour of every already roughly aligned point
-    int rc = nns_build(&c->nns, target_dev, c->point ? nullptr : target_normals_dev, m, options->max_correspondence_distance,
+    int rc = nns_build(&c->nns, target_dev, c->est == kEstPoint ? nullptr : target_normals_dev, m,
+                       options->max_correspondence_distance,
                        options->cell_scale > 0 ? options->cell_scale : kDefaultCellScale, st);
     if (rc) return rc;
     for (int k = 0; k < 3; ++k)   // (Grid::bmin / bmax are in grid-axis order: grid axis k is world axis ax[k])
@@ -2626,34 +2628,29 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     // fitness denominator over all ranks
     c->n_total = (double)n;
     int occ = 1;
-    for (int mode = 0; mode < 2; ++mode)
-        O3DB_CUDA_CHECK(cudaFuncSetAttribute(icp_kernel_for(c.get(), mode), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)icp_smem_bytes(c.get(), mode)));
-    O3DB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, icp_kernel_for(c.get(), 0), kIcpThreads,
-                                                                  icp_smem_bytes(c.get(), 0)));
+    for (int mode = 0; mode < 2; ++mode) {
+        const IcpLaunch k = icp_launch_for(c.get(), mode);
+        O3DB_CUDA_CHECK(cudaFuncSetAttribute(k.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem));
+    }
+    const IcpLaunch it = icp_launch_for(c.get(), 0);
+    O3DB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, it.kernel, kIcpThreads, it.smem));
     c->grid_blocks = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, kIcpThreads), (int64_t)num_sms() * std::max(occ, 1)));
     const int64_t ncell = tiled_key_space(c->nns.g.nx, c->nns.g.ny, c->nns.g.nz);   // tile-major source keys
-    c->src_keys = ncell;
     // padded to whole 256-entry chunks: the staged kernel copies 32-entry chunks with TMA bulk copies
     c->n_pad = ceil_div(n, 256) * 256;
-    if ((rc = dev_alloc(c->src_blk, c->symmetric ? SrcBlockedSym::bytes(c->n_pad)
-                                    : c->doppler ? SrcBlockedDop::bytes(c->n_pad) : SrcBlocked::bytes(c->n_pad), st)))
-        return rc;
+    const size_t src_bytes = with_estimator(c->est, [&](auto e) { return SrcOf<decltype(e)::value>::bytes(c->n_pad); });
+    if ((rc = dev_alloc(c->src_blk, src_bytes, st))) return rc;
     if ((rc = dev_alloc(c->src_idx, (size_t)c->n_pad, st))) return rc;
     // (no initial contents: IcpState::sums_cached starts at 0, so the first iteration writes every line)
     if ((rc = dev_alloc(c->chunk_sums, (size_t)c->n_pad, st))) return rc;
-    if (c->symmetric) {
+    if (c->est == kEstSymmetric) {
         if ((rc = dev_alloc(c->chunk_sums2, (size_t)(c->n_pad / 32) * kSymLine2, st))) return rc;
         if ((rc = dev_alloc(c->partials2, (size_t)c->grid_blocks * kSymLine2, st))) return rc;
-        src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlockedSym{c->src_blk.get()},
-                                                                                           n, c->n_pad, true);
-    } else if (c->doppler) {
-        src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlockedDop{c->src_blk.get()},
-                                                                                           n, c->n_pad, true);
-    } else {
-        src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(SrcBlocked{c->src_blk.get()}, n,
-                                                                                           c->n_pad, true);
     }
+    with_estimator(c->est, [&](auto e) {
+        src_blocked_init_kernel<<<(unsigned)ceil_div(c->n_pad, kThreads), kThreads, 0, st>>>(
+                SrcOf<decltype(e)::value>{c->src_blk.get()}, n, c->n_pad, true);
+    });
     O3DB_LAUNCH_CHECK();
     const size_t iter_sums = (size_t)std::max(1, options->max_iteration) * 2;
     if ((rc = dev_alloc(c->src_key, (size_t)n, st))) return rc;
@@ -2685,7 +2682,7 @@ static int icp_create_impl(const float* source_dev, int64_t n, const float* targ
     scratch.reset();
     if ((rc = canonical_ranks(n, c->src_start.get(), c->src_key.get(), c->src_rank.get(), st))) return rc;
     if ((rc = icp_gather_source(c.get(), st))) return rc;
-    if (c->colored) {
+    if (c->est == kEstColored) {
         if ((rc = dev_alloc(c->tcg4, (size_t)m, st))) return rc;
         if ((rc = dev_alloc(c->sint, (size_t)n, st))) return rc;
         pack_target_color_kernel<<<(unsigned)ceil_div(m, kThreads), kThreads, 0, st>>>(
@@ -2715,7 +2712,7 @@ int o3db_icp_create(const float* source_dev, int64_t n, const float* target_dev,
                     int64_t m, const double init_T[16], const o3db_icp_options* options, o3db_comm* comm,
                     void* stream, o3db_icp** out) {
     return icp_create_impl(source_dev, n, target_dev, target_normals_dev, m, init_T, options, comm,
-                           o3db::EstimatorInputs{}, stream, out);
+                           o3db::EstimatorInputs{kEstPlane}, stream, out);
 }
 
 int o3db_icp_create_colored(const float* source_dev, const float* source_colors_dev, int64_t n,
@@ -2731,7 +2728,7 @@ int o3db_icp_create_colored(const float* source_dev, const float* source_colors_
     O3DB_REQUIRE(target_color_gradients_dev != nullptr,
                  "Target pointcloud missing color_gradients attribute (o3db_estimate_color_gradients).");
     O3DB_REQUIRE(lambda_geometric >= 0.0 && lambda_geometric <= 1.0, "lambda_geometric must be in [0, 1]");
-    o3db::EstimatorInputs col;
+    o3db::EstimatorInputs col{kEstColored};
     col.source_colors = source_colors_dev;
     col.target_colors = target_colors_dev;
     col.target_color_gradients = target_color_gradients_dev;
@@ -2742,9 +2739,8 @@ int o3db_icp_create_colored(const float* source_dev, const float* source_colors_
 int o3db_icp_create_point_to_point(const float* source_dev, int64_t n, const float* target_dev, int64_t m,
                                    const double init_T[16], const o3db_icp_options* options, o3db_comm* comm, void* stream,
                                    o3db_icp** out) {
-    o3db::EstimatorInputs est;
-    est.point_to_point = true;
-    return icp_create_impl(source_dev, n, target_dev, nullptr, m, init_T, options, comm, est, stream, out);
+    return icp_create_impl(source_dev, n, target_dev, nullptr, m, init_T, options, comm, o3db::EstimatorInputs{kEstPoint},
+                           stream, out);
 }
 
 int o3db_icp_create_symmetric(const float* source_dev, const float* source_normals_dev, int64_t n, const float* target_dev,
@@ -2758,7 +2754,7 @@ int o3db_icp_create_symmetric(const float* source_dev, const float* source_norma
                  "SymmetricICP requires both source and target to have normals.");
     // the in-kernel exchange and the NCCL path carry the 30 sums of one line; this estimator has a second line
     O3DB_REQUIRE(comm == nullptr, "SymmetricICP does not run multi-GPU: pass no communicator.");
-    o3db::EstimatorInputs est;
+    o3db::EstimatorInputs est{kEstSymmetric};
     est.source_normals = source_normals_dev;
     return icp_create_impl(source_dev, n, target_dev, target_normals_dev, m, init_T, options, nullptr, est, stream, out);
 }
@@ -2780,7 +2776,7 @@ int o3db_icp_create_doppler(const float* source_dev, const float* source_doppler
     O3DB_REQUIRE(comm == nullptr, "DopplerICP does not run multi-GPU: pass no communicator.");
     o3db::DopplerConst k;
     if (int rc = o3db::doppler_const(params, options->max_iteration, &k)) return rc;
-    o3db::EstimatorInputs est;
+    o3db::EstimatorInputs est{kEstDoppler};
     est.source_dopplers = source_dopplers_dev;
     est.source_directions = source_directions_dev;
     est.dop = &k;
@@ -2870,45 +2866,41 @@ int o3db_icp_state(o3db_icp* c, o3db_icp_result* result, double* per_iteration_h
     return icp_read_state(c, result, per_iteration_host, (cudaStream_t)stream);
 }
 
+// The one-shot entry points after a successful create: every iteration of the handle's options, the final evaluation
+// unless an iteration failed, and the handle's destruction once the stream has drained.
+static int icp_run_to_end(o3db_icp* c, o3db_icp_result* result, int64_t* correspondences_dev, double* per_iteration_host,
+                          void* stream) {
+    int rc = o3db_icp_iterate(c, c->opt.max_iteration, stream);
+    if (rc == O3DB_OK) rc = o3db_icp_finish(c, result, correspondences_dev, per_iteration_host, stream);
+    cudaStreamSynchronize((cudaStream_t)stream);
+    o3db_icp_destroy(c);
+    return rc;
+}
+
 int o3db_icp_point_to_plane(const float* source_dev, int64_t n, const float* target_dev,
                             const float* target_normals_dev, int64_t m, const double init_T[16],
                             const o3db_icp_options* options, o3db_icp_result* result, int64_t* correspondences_dev,
                             double* per_iteration_host, void* stream) {
     o3db_icp* c = nullptr;
-    int rc = o3db_icp_create(source_dev, n, target_dev, target_normals_dev, m, init_T, options, nullptr, stream, &c);
-    if (rc) return rc;
-    rc = o3db_icp_iterate(c, options->max_iteration, stream);
-    if (rc == O3DB_OK) rc = o3db_icp_finish(c, result, correspondences_dev, per_iteration_host, stream);
-    cudaStreamSynchronize((cudaStream_t)stream);
-    o3db_icp_destroy(c);
-    return rc;
+    const int rc = o3db_icp_create(source_dev, n, target_dev, target_normals_dev, m, init_T, options, nullptr, stream, &c);
+    return rc ? rc : icp_run_to_end(c, result, correspondences_dev, per_iteration_host, stream);
 }
 
 int o3db_icp_point_to_point(const float* source_dev, int64_t n, const float* target_dev, int64_t m, const double init_T[16],
                             const o3db_icp_options* options, o3db_icp_result* result, int64_t* correspondences_dev,
                             double* per_iteration_host, void* stream) {
     o3db_icp* c = nullptr;
-    int rc = o3db_icp_create_point_to_point(source_dev, n, target_dev, m, init_T, options, nullptr, stream, &c);
-    if (rc) return rc;
-    rc = o3db_icp_iterate(c, options->max_iteration, stream);
-    if (rc == O3DB_OK) rc = o3db_icp_finish(c, result, correspondences_dev, per_iteration_host, stream);
-    cudaStreamSynchronize((cudaStream_t)stream);
-    o3db_icp_destroy(c);
-    return rc;
+    const int rc = o3db_icp_create_point_to_point(source_dev, n, target_dev, m, init_T, options, nullptr, stream, &c);
+    return rc ? rc : icp_run_to_end(c, result, correspondences_dev, per_iteration_host, stream);
 }
 
 int o3db_icp_symmetric(const float* source_dev, const float* source_normals_dev, int64_t n, const float* target_dev,
                        const float* target_normals_dev, int64_t m, const double init_T[16], const o3db_icp_options* options,
                        o3db_icp_result* result, int64_t* correspondences_dev, double* per_iteration_host, void* stream) {
     o3db_icp* c = nullptr;
-    int rc = o3db_icp_create_symmetric(source_dev, source_normals_dev, n, target_dev, target_normals_dev, m, init_T, options,
-                                       nullptr, stream, &c);
-    if (rc) return rc;
-    rc = o3db_icp_iterate(c, options->max_iteration, stream);
-    if (rc == O3DB_OK) rc = o3db_icp_finish(c, result, correspondences_dev, per_iteration_host, stream);
-    cudaStreamSynchronize((cudaStream_t)stream);
-    o3db_icp_destroy(c);
-    return rc;
+    const int rc = o3db_icp_create_symmetric(source_dev, source_normals_dev, n, target_dev, target_normals_dev, m, init_T,
+                                             options, nullptr, stream, &c);
+    return rc ? rc : icp_run_to_end(c, result, correspondences_dev, per_iteration_host, stream);
 }
 
 int o3db_icp_doppler(const float* source_dev, const float* source_dopplers_dev, const float* source_directions_dev, int64_t n,
@@ -2916,14 +2908,9 @@ int o3db_icp_doppler(const float* source_dev, const float* source_dopplers_dev, 
                      const o3db_icp_options* options, const o3db_doppler_params* params, o3db_icp_result* result,
                      int64_t* correspondences_dev, double* per_iteration_host, void* stream) {
     o3db_icp* c = nullptr;
-    int rc = o3db_icp_create_doppler(source_dev, source_dopplers_dev, source_directions_dev, n, target_dev,
-                                     target_normals_dev, m, init_T, options, params, nullptr, stream, &c);
-    if (rc) return rc;
-    rc = o3db_icp_iterate(c, options->max_iteration, stream);
-    if (rc == O3DB_OK) rc = o3db_icp_finish(c, result, correspondences_dev, per_iteration_host, stream);
-    cudaStreamSynchronize((cudaStream_t)stream);
-    o3db_icp_destroy(c);
-    return rc;
+    const int rc = o3db_icp_create_doppler(source_dev, source_dopplers_dev, source_directions_dev, n, target_dev,
+                                           target_normals_dev, m, init_T, options, params, nullptr, stream, &c);
+    return rc ? rc : icp_run_to_end(c, result, correspondences_dev, per_iteration_host, stream);
 }
 
 int o3db_icp_colored(const float* source_dev, const float* source_colors_dev, int64_t n, const float* target_dev,
@@ -2932,15 +2919,10 @@ int o3db_icp_colored(const float* source_dev, const float* source_colors_dev, in
                      const o3db_icp_options* options, double lambda_geometric, o3db_icp_result* result,
                      int64_t* correspondences_dev, double* per_iteration_host, void* stream) {
     o3db_icp* c = nullptr;
-    int rc = o3db_icp_create_colored(source_dev, source_colors_dev, n, target_dev, target_normals_dev,
-                                     target_colors_dev, target_color_gradients_dev, m, init_T, options,
-                                     lambda_geometric, nullptr, stream, &c);
-    if (rc) return rc;
-    rc = o3db_icp_iterate(c, options->max_iteration, stream);
-    if (rc == O3DB_OK) rc = o3db_icp_finish(c, result, correspondences_dev, per_iteration_host, stream);
-    cudaStreamSynchronize((cudaStream_t)stream);
-    o3db_icp_destroy(c);
-    return rc;
+    const int rc = o3db_icp_create_colored(source_dev, source_colors_dev, n, target_dev, target_normals_dev,
+                                           target_colors_dev, target_color_gradients_dev, m, init_T, options,
+                                           lambda_geometric, nullptr, stream, &c);
+    return rc ? rc : icp_run_to_end(c, result, correspondences_dev, per_iteration_host, stream);
 }
 
 int o3db_icp_point_to_plane_host(const float* source_host, int64_t n, const float* target_host,
@@ -2984,16 +2966,13 @@ int o3db_icp_point_to_plane_host(const float* source_host, int64_t n, const floa
     O3DB_CUDA_CHECK(cudaStreamWaitEvent(copy_stream, buffers_ready, 0));      // d_src exists (stream-ordered allocation)
     O3DB_CUDA_CHECK(cudaMemcpyAsync(d_src.get(), source_host, n * 3 * sizeof(float), cudaMemcpyHostToDevice, copy_stream));
     O3DB_CUDA_CHECK(cudaEventRecord(source_ready, copy_stream));
-    o3db_icp* raw = nullptr;
-    int rc = icp_create_impl(d_src.get(), n, d_tgt.get(), d_nrm.get(), m, init_T, options, nullptr, o3db::EstimatorInputs{},
-                             st, &raw, source_ready);
-    std::unique_ptr<o3db_icp, HandleDestroy<o3db_icp_destroy>> c(raw);
+    o3db_icp* c = nullptr;
+    int rc = icp_create_impl(d_src.get(), n, d_tgt.get(), d_nrm.get(), m, init_T, options, nullptr,
+                             o3db::EstimatorInputs{kEstPlane}, st, &c, source_ready);
     // whatever fails, the source copy and the kernels finish before the buffers are freed
-    if (rc == O3DB_OK) rc = o3db_icp_iterate(c.get(), options->max_iteration, st);
-    if (rc == O3DB_OK) rc = o3db_icp_finish(c.get(), result, d_corr.get(), per_iteration_host, st);
-    cudaStreamSynchronize(st);
+    if (rc == O3DB_OK) rc = icp_run_to_end(c, result, d_corr.get(), per_iteration_host, st);
+    else cudaStreamSynchronize(st);
     cudaStreamSynchronize(copy_stream);
-    c.reset();
     if (rc) return rc;
     if (correspondences_host) {
         O3DB_CUDA_CHECK(cudaMemcpyAsync(correspondences_host, d_corr.get(), n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
